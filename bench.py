@@ -1,13 +1,13 @@
 #!/usr/bin/env python
-"""Benchmark of the TokenPacker projector hot path on B200 (contract: see the task brief / DESIGN.md §Measurement).
+"""Benchmark of the TokenPacker projector hot path on an H100 (see DESIGN.md §Measurement).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload projector|hd5|train]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload projector|hd5|train] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 One "step" = one TokenPacker.forward over one batch of synthetic CLIP features per GPU.  Workload at every N:
 BASELINE.json configs[1] per GPU — batch=64 crops of 576x1024 (+576x4096 multi-level) bf16 features, scale_factor=2,
 hidden=4096 -> 9,216 compressed tokens per GPU per step (weak scaling: crops shard across ranks, no data-path
-collective; weights replicated).  Prints ONE JSON line on rank 0.  Besides the contract's keys the line carries:
+collective; weights replicated).  Prints ONE JSON line on rank 0.  Besides the headline keys the line carries:
   sustained  the same step for >= 2 s with clocks sampled inside the region (power-capped regime), rated against the sustained peak
   hd5        (N > 1) BASELINE configs[4]: 256 HD crops, s=4, sharded across the ranks, packed per-image sequences on every rank:
              NCCL all-gather + assembly vs the fused peer-store GEMM, strong-scaling efficiency, bit-exactness vs one GPU
@@ -42,12 +42,13 @@ def load_peaks():
         p = json.load(open(path))
         return {"hbm_gbs": p["hbm_gbs"], "bf16_burst": p["bf16_tflops"], "bf16_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_burst": 1590.0, "bf16_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s — a ceiling to rate against, never reached
+    return {"hbm_gbs": 3350.0, "bf16_burst": 989.0, "bf16_sustained": 989.0, "source": "H100 SXM data sheet (700 W)"}
 
 
 class ClockSampler:
     """SM clock / throttle-reason sampling DURING the timed region.  NVML is polled from a thread (~1 kHz, so that even a 20 ms
-    region holds a dozen samples); nvidia-smi -lms (B200_PROFILING.md recipe) is the fallback.  Samples carry their own
+    region holds a dozen samples); nvidia-smi -lms is the fallback.  Samples carry their own
     timestamps and are filtered to the timed window."""
     Q = "timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -202,17 +203,15 @@ def cpu_reference_run(steps: int, warmup: int, crops: int):
             torch_port.forward(params, x0[:1], xm[:1], SCALE)
         single_ms = (time.perf_counter() - t0) / 5 * 1e3
     return {"value": crops * TOKENS_PER_CROP / dt, "unit": UNIT, "cores": int(torch.get_num_threads()), "kind": "port",
-            "pinned": "oracle/torch_port.py is held to fixtures generated by the reference module itself (tests/golden, < 1e-6) and to live "
-                      "runs of the reference where /root/reference is mounted (tests/test_reference_live.py)",
+            "pinned": "oracle/torch_port.py is held to fixtures generated by the reference module itself (tests/golden, < 1e-6)",
             "configs0_single_image_ms": single_ms,
             "sample": f"{crops} crops/step x {steps} steps of the configs[1] workload (fp32, torch {torch.__version__} CPU ops, "
                       f"oracle/torch_port.py restatement of builder.py:107-137; best of pool sizes {cands} on {avail} visible cores), {dt * 1e3:.1f} ms/step"}, dt
 
 
 def run_reference(args):
-    """--impl reference: the reference's CPU implementation of the path (the pinned PyTorch-CPU port; /root/reference is
-    not present on the GPU box and the reference is pure Python) on the host cores, same metric/config: the full configs[1]
-    batch (64 crops) per step."""
+    """--impl reference: the reference's CPU implementation of the path (the pinned PyTorch-CPU port: the reference itself is
+    pure Python and not a dependency) on the host cores, same metric/config: the full configs[1] batch (64 crops) per step."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -469,6 +468,19 @@ def hd_tile_measure(dev, peaks):
             "achieved_gbs": bytes_alg / (ms * 1e-3) / 1e9, "peak_gbs": peaks["hbm_gbs"], "frac": bytes_alg / (ms * 1e-3) / 1e9 / peaks["hbm_gbs"]}
 
 
+DUMP_ROWS = 2048
+
+
+def dump_outputs(out_dir, out):
+    """The timed path's result of its last step, [crops, tokens, hidden] bf16: a fixed seeded sample of DUMP_ROWS token rows
+    (all of them would be 151 MB as float32), in ascending row order, as float32."""
+    os.makedirs(out_dir, exist_ok=True)
+    flat = out.reshape(-1, out.shape[-1])
+    rows = np.sort(np.random.default_rng(0).choice(flat.shape[0], size=min(DUMP_ROWS, flat.shape[0]), replace=False))
+    sample = flat[torch.from_numpy(rows).to(flat.device)].float().cpu().numpy()
+    np.save(os.path.join(out_dir, "projector_out.npy"), sample)
+
+
 def bind_numa(local_rank):
     try:
         from tokenpacker_b200.numa import bind_to_gpu_node
@@ -484,13 +496,18 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="projector", choices=["projector", "hd5", "train"],
-                    help="projector: BASELINE configs[1] (default, the driver's line; carries hd5 at N > 1 and train at N = 1 as records); "
+                    help="projector: BASELINE configs[1] (default; carries hd5 at N > 1 and train at N = 1 as records); "
                          "hd5: configs[4] HD reassembly across ranks as its own line; train: forward + backward as its own line")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip the CPU baseline leg (profiling runs)")
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-buffer end-to-end leg (profiling runs)")
     ap.add_argument("--no-extras", action="store_true", help="skip the sustained / hd5 / train / eager records (profiling runs)")
     ap.add_argument("--sustained-seconds", type=float, default=2.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help=f"projector workload: after the timed steps write the last step's output as DIR/projector_out.npy (float32 "
+                         f"[{DUMP_ROWS}, hidden]: a fixed seeded sample of the batch's token rows) so that two builds can be compared")
     args = ap.parse_args()
+    if args.dump_outputs is not None and (args.impl != "ours" or args.workload != "projector"):
+        ap.error("--dump-outputs applies to the projector workload of --impl ours")
     args.warmup = max(args.warmup, 3)
 
     if args.impl == "reference":
@@ -504,7 +521,7 @@ def main():
         if world == 1 and args.gpus > 1:
             raise SystemExit("launch multi-GPU runs with torch.distributed.run (one process per GPU)")
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py --impl ours needs a B200: tokenpacker_b200 has no CPU path")
+        raise SystemExit("bench.py --impl ours needs an H100: tokenpacker_b200 has no CPU path")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     # host placement BEFORE any pinned allocation: this rank's CPU threads (and therefore its first-touch pinned buffers) go to the
@@ -537,7 +554,7 @@ def main():
     xm = torch.randn(N_CROPS, 576, 4096, device=dev, generator=g).to(torch.bfloat16)
 
     if args.workload == "train":
-        rec = train_measure(model, x0, xm, steps=max(3, min(args.steps, 50)))
+        rec = train_measure(model, x0, xm, steps=args.steps)
         if rank == 0:
             print(json.dumps({"metric": "projector_train_step_ms", "value": rec["fwd_bwd_ms"], "unit": "ms", "n_gpus": world, "steps": rec["steps"],
                               "warmup": 3, "ms_per_step": rec["fwd_bwd_ms"], "higher_is_better": False, "scaling": "weak", "dtype": "bf16",
@@ -587,6 +604,8 @@ def main():
         ms_per_step, clocks, launches, out = timed_steps(args.steps, True)
     value = tokens_per_step / (ms_per_step * 1e-3)
     assert torch.isfinite(out.float()).all()
+    if args.dump_outputs is not None and rank == 0:
+        dump_outputs(args.dump_outputs, out)
     region_s = ms_per_step * args.steps * 1e-3
     regime = "sustained" if region_s >= 1.0 else "burst"
 
@@ -613,7 +632,7 @@ def main():
                 model.forward_host((hx0, hxm), out=hout, chunk_crops=8)
             barrier()
             t0 = time.perf_counter()
-            e2e_steps = min(args.steps, 100)       # PCIe-bound at ~7.4 ms/step: 100 steps are plenty
+            e2e_steps = min(args.steps, 100)       # PCIe-bound, several ms per step: 100 steps are plenty
             for _ in range(e2e_steps):
                 model.forward_host((hx0, hxm), out=hout, chunk_crops=8)      # synchronous: result is in hout on return
             torch.cuda.synchronize()
@@ -661,16 +680,12 @@ def main():
         k_ms = r0.elapsed_time(r1) / reps
         flops = 2.0 * m_ * n_ * k_
         achieved = flops / (k_ms * 1e-3) / 1e12
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "dominant_kernel_traffic.json")
-        if os.path.exists(tpath):
-            traffic = json.load(open(tpath)).get("dram_bytes_per_launch")
         step_tf = flops_step / (ms_per_step * 1e-3) / 1e12
         step_peak = peaks["bf16_sustained"] if regime == "sustained" else peaks["bf16_burst"]
-        roofline = {"bound": "tensor", "kernel": "tp_gemm2_kernel (CTA-pair tcgen05 GEMM; largest launch: k/v_proj.0, M=36864 N=2048 K=4096, bias+GELU epilogue)",
+        roofline = {"bound": "tensor", "kernel": "tp_gemm2_kernel (wgmma GEMM, 256 x 256 tiles; largest launch: k/v_proj.0, M=36864 N=2048 K=4096, bias+GELU epilogue)",
                     "achieved": achieved, "peak": peaks["bf16_burst"], "unit": "TFLOP/s", "frac": achieved / peaks["bf16_burst"],
                     "peak_source": peaks["source"] + ": burst figure (this kernel is timed alone, 10 launches)",
-                    "traffic": traffic, "ms_per_launch": k_ms, "flops_per_launch": flops,
+                    "ms_per_launch": k_ms, "flops_per_launch": flops,
                     "step": {"what": f"whole step of the timed `value` region ({args.steps} steps, {region_s * 1e3:.0f} ms: a {regime} measurement, rated against the "
                                      f"{regime} peak; the >= 2 s run is in `sustained`)",
                              "achieved_tflops": step_tf, "peak": step_peak, "regime": regime, "frac": step_tf / step_peak,
@@ -684,8 +699,8 @@ def main():
         hd5 = hd5_measure(max(5, min(args.steps, 50)), 5, rank, world, dev, dist)
 
     # ------------------------------------------------------------------ the reference's op sequence, eager on THIS GPU
-    # (SURVEY.md §8d "second baseline": the reference ships no Blackwell kernel, so its own ATen/cuBLAS eager path on the same
-    # box is the real bar.)  oracle/torch_port.py = the reference forward as PyTorch ops in the reference's order; bf16.
+    # (SURVEY.md §8d "second baseline": the reference ships no kernel of its own, so its ATen/cuBLAS eager path on the same
+    # GPU is the real bar.)  oracle/torch_port.py = the reference forward as PyTorch ops in the reference's order; bf16.
     gpu_eager = None
     if rank == 0 and world == 1 and not args.no_cpu_baseline and not args.no_extras:
         from oracle import torch_port
@@ -704,7 +719,7 @@ def main():
         diff = (ref_out.float() - out.float())
         gpu_eager = {"value": N_CROPS * TOKENS_PER_CROP / (g_ms * 1e-3), "unit": UNIT, "ms_per_step": g_ms, "kind": "port",
                      "what": "oracle/torch_port.py (reference op sequence: F.linear/gelu/layer_norm/interpolate/multi_head_attention_forward) "
-                             "eager bf16 on the same B200, same weights and inputs",
+                             "eager bf16 on the same GPU, same weights and inputs",
                      "rel_rms_vs_ours": float(diff.pow(2).mean().sqrt() / ref_out.float().pow(2).mean().sqrt())}
         del ref_out
 
@@ -757,7 +772,7 @@ def main():
                 "config": {"workload": "BASELINE configs[1] per GPU: batch=64 crops, CLIP-ViT-L/14-336 feats 576x1024 + 576x4096, "
                                        "scale_factor=2 (144 tok/crop), hidden=4096, bf16, seeded random weights",
                            "crops_per_gpu": N_CROPS, "tokens_per_step": tokens_per_step,
-                           "l2": "inputs 377 MB/step per GPU exceed the 126 MB L2 (no explicit flush needed)",
+                           "l2": "inputs 377 MB/step per GPU exceed the 50 MB L2 (no explicit flush needed)",
                            "parallelism": f"dp{world} (crops sharded, weights replicated, no data-path collective)"},
                 "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "roofline": roofline, "sustained": sustained, "hd5": hd5,
                 "train": train, "hd_tile": hd_tile, "cpu_baseline": cpu_baseline, "gpu_eager_baseline": gpu_eager, "configs0_single_image": single}

@@ -1,4 +1,4 @@
-/* tokenpacker_b200 — C ABI of the B200-native TokenPacker hot path (libtokenpacker_b200.so).
+/* tokenpacker_b200 — C ABI of the H100 (sm_90a) TokenPacker hot path (libtokenpacker_b200.so).
  *
  * The reference (CircleRadon/TokenPacker) is pure Python and has no FFI of its own: its boundary for this path is
  * the nn.Module ``TokenPacker`` (llava/model/multimodal_projector/builder.py:39-137) plus the HD front end

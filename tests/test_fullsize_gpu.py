@@ -4,8 +4,8 @@ sequence, builder.py:107-137, in full fp32 arithmetic — the port is pinned to 
 reference by tests/test_oracle.py / tests/test_reference_live.py).  EVERY output row is compared.
 
 Tolerances (bf16 storage + fp32 accumulation vs the fp32 oracle on identical bf16-rounded weights and inputs, output RMS ~0.1):
-forward rel-RMS <= 4e-3 and max-abs <= 5e-3 at H=4096 (measured on a B200: 3.4e-3 / 3.8e-3 at N=64 with k' / v' rounded to bf16;
-the error grows with the width of the last two linears — 2.1e-3 / 1.3e-3 at H=256 — and the reference's own bf16 forward sits at
+forward rel-RMS <= 4e-3 and max-abs <= 5e-3 at H=4096 (the error grows with the width of the last two linears — 2.0e-3 / 1.3e-3
+at H=256, measured on an H100 — and the reference's own bf16 forward sits at
 4.6e-3..5.3e-3 / up to 4.9e-3 on the same inputs); parameter gradients at H=4096, N=8: <= 1.5 % rel-RMS each.
 """
 import numpy as np

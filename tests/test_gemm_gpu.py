@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (tp_gemm_bf16 through the C ABI) against a plain PyTorch fp32 reference of the same op."""
+"""wgmma GEMM (tp_gemm_bf16 through the C ABI) against a plain PyTorch fp32 reference of the same op."""
 import pytest
 import torch
 

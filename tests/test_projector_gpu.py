@@ -1,7 +1,7 @@
-"""Parity of the CUDA projector (through the nn.Module -> C ABI -> sm_100a kernels) with the oracle and the
+"""Parity of the CUDA projector (through the nn.Module -> C ABI -> sm_90a kernels) with the oracle and the
 reference-generated golden fixtures.  Tolerances (stated per SURVEY.md §8c): bf16 storage / fp32 accumulation vs the
-fp32|fp64 oracle on identical bf16-rounded weights and inputs: rel-RMS <= 4e-3 and max-abs <= 5e-3 (measured on B200: 2.0e-3 / 1.3e-3 at
-hidden 256, 3.1e-3..3.4e-3 / 3.6e-3..3.9e-3 at hidden 4096 / 5120: the error grows with the width of the last two linears) at output
+fp32|fp64 oracle on identical bf16-rounded weights and inputs: rel-RMS <= 4e-3 and max-abs <= 5e-3 (measured on an H100: 2.0e-3 / 1.3e-3 at
+hidden 256; the error grows with the width of the last two linears) at output
 RMS ~0.1 (the reference's own bf16-vs-fp32 gap at these inputs is rel-RMS 4.6e-3..5.3e-3, max-abs up to 4.9e-3)."""
 import os
 
@@ -205,7 +205,7 @@ def test_fused_single_launch_vs_separate_kernels(s, hidden, n, monkeypatch):
         rel, mx = errors(out.float().cpu().numpy(), ref)
         assert rel <= REL_RMS_TOL and mx <= MAX_ABS_TOL, (name, rel, mx)
     d = (fused.float() - plain.float())
-    # the two plans differ by the bf16 rounding of k' / v' (and the summation order inside a window): measured 1.7e-3 .. 3.2e-3
+    # the two plans differ by the bf16 rounding of k' / v' (and the summation order inside a window)
     assert float(d.pow(2).mean().sqrt() / plain.float().pow(2).mean().sqrt()) < 4e-3
 
 

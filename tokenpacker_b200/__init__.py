@@ -1,8 +1,8 @@
-"""tokenpacker_b200 — B200-native (sm_100a) implementation of the TokenPacker visual projector hot path.
+"""tokenpacker_b200 — H100 (sm_90a) implementation of the TokenPacker visual projector hot path.
 
 Drop-in for ``llava/model/multimodal_projector/builder.py`` of CircleRadon/TokenPacker:
 ``build_vision_projector(config)`` / ``TokenPackerB200.forward((feat, feat_multi))`` keep the reference's
-constructor, parameter names and output layout; the arithmetic runs in hand-written tcgen05/TMA CUDA kernels behind
+constructor, parameter names and output layout; the arithmetic runs in hand-written wgmma/TMA CUDA kernels behind
 the C ABI declared in ``include/tokenpacker_b200.h``.  There is no CPU fallback.
 """
 from . import _lib  # noqa: F401  (fails loudly when the CUDA library is not built)

@@ -138,7 +138,7 @@ int device_info(DeviceInfo* info) {
   int dev = 0, major = 0;
   TP_CUDA(cudaGetDevice(&dev));
   TP_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (major != 10) return TP_ERR_UNSUPPORTED_DEVICE;
+  if (major != 9) return TP_ERR_UNSUPPORTED_DEVICE;
   TP_CUDA(cudaDeviceGetAttribute(&info->sms, cudaDevAttrMultiProcessorCount, dev));
   return TP_OK;
 }
@@ -156,7 +156,7 @@ struct AOperand {
 };
 
 // Every kernel of the path is launched with the programmatic-stream-serialization attribute (PDL): its CTAs may be
-// scheduled while the previous kernel on the stream drains, run their prologue (barrier init, TMEM allocation, tensor-map
+// scheduled while the previous kernel on the stream drains, run their prologue (barrier init, tensor-map
 // prefetch) and then block in griddepcontrol.wait until the previous kernel's memory is visible.
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
@@ -511,19 +511,23 @@ int choose_kernel(const GemmItem& it, int count, int sms, int mode) {
   const bool pair_only = it.n_peers > 0 || it.tn || it.ep.dual || it.a.parts > 1 || it.k_splits > 1 || it.ep.out_f32 || it.kind == 1 || it.ep.wm_s != 0;   // pair-kernel-only features
   if (pair_only && !pair_ok) return -1;
   const bool needs_256 = it.ep.stats_out != nullptr;                        // statistics slots assume 256-column tiles
-  // Estimated tensor-pipe cycles of each candidate = waves x k-blocks x cycles per k-block.  Large problems always land
-  // on the pair kernel; small ones (single crops: the serving latency case) get the tile shape that fills more SMs.  All
-  // kernels produce identical bits, so the choice never changes results.
+  // Estimated tensor-pipe cycles of each candidate = waves x k-blocks x cycles per k-block of one CTA.  An H100 SM does 4096 dense
+  // bf16 FLOP per cycle (989 TFLOP/s over 132 SMs at 1.83 GHz), so a 128 x 256 x 64 k-block takes 1024 cycles and a 128 x 128 x 64
+  // one 512; a pair tile is two CTAs of 128 x 256 side by side.  Large problems always land on the pair kernel; small ones
+  // (single crops: the serving latency case) get the tile shape that fills more SMs.  All kernels produce identical bits, so the
+  // choice never changes results.
   const long long kb = (it.K + kBlockK - 1) / kBlockK;
   auto waves = [](long long tiles, long long units) { return (tiles + units - 1) / units; };
   const long long t_pair = ((it.M + 255) / 256) * ((it.N + 255) / 256);
   const long long t_256 = ((it.M + 127) / 128) * ((it.N + 255) / 256);
   const long long t_128 = ((it.M + 127) / 128) * ((it.N + 127) / 128);
-  const long long c_pair = pair_ok ? waves(t_pair, sms / 2) * kb * 512 : LLONG_MAX;
-  // one-CTA kernels pay ~40 % over their nominal MMA time (more operand traffic per FLOP, direct 16-byte stores, no grouping):
-  // measured — at 10 crops the nominally 16 % cheaper 128x128 tiling was 30 % slower than the pair kernel
-  const long long c_256 = (it.N % 256 == 0) ? waves(t_256, sms) * kb * 512 * 14 / 10 : LLONG_MAX;
-  const long long c_128 = needs_256 ? LLONG_MAX : waves(t_128, sms) * kb * 256 * 14 / 10;
+  // The pair kernel's ring is one stage shallower (3 x 48 KiB next to its output slabs, against 4 in the one-CTA kernels): on an
+  // H100 at equal waves it ran 10 - 25 % behind the one-CTA 128 x 256 kernel (bias + GELU GEMMs, M = 576 .. 36864 rows, N = 1024 /
+  // 2048, K = 1024 / 4096), so it is charged 1/8 over its nominal MMA time.  The 128-wide kernel reads every A tile once per 128
+  // columns instead of per 256: at 36864 x 2048 x 4096 it took 1.21x the 256-wide kernel's time at equal waves, so it is charged 1/5.
+  const long long c_pair = pair_ok ? waves(t_pair, sms / 2) * kb * 1024 * 9 / 8 : LLONG_MAX;
+  const long long c_256 = (it.N % 256 == 0) ? waves(t_256, sms) * kb * 1024 : LLONG_MAX;
+  const long long c_128 = needs_256 ? LLONG_MAX : waves(t_128, sms) * kb * 512 * 6 / 5;
   // a launch costs ~10k cycles of ramp and drain; pair-kernel items of one call share a single (grouped) launch
   const long long launch = 10000;
   const long long l_pair = pair_ok ? c_pair + launch / count : LLONG_MAX;
@@ -831,7 +835,7 @@ const char* tp_strerror(int status) {
     case TP_ERR_BAD_SCALE_FACTOR: return "scale_factor must be divisible by grid size";   // builder.py:52 message
     case TP_ERR_WORKSPACE_TOO_SMALL: return "workspace too small";
     case TP_ERR_CUDA: return "CUDA error";
-    case TP_ERR_UNSUPPORTED_DEVICE: return "unsupported device: tokenpacker_b200 needs an sm_100a (B200) GPU";
+    case TP_ERR_UNSUPPORTED_DEVICE: return "unsupported device: tokenpacker_b200 needs an sm_90a (H100) GPU";
     case TP_ERR_BAD_PATCH_NUM: return "patch_num must be 9, 16 or 25";
     default: return "unknown status";
   }
@@ -1130,8 +1134,8 @@ int forward_impl(const void* packed, const void* x0, const void* xm, const void*
       //   3: see below (wavefront over the last three stages only; for the fused all-gather).
       //   4, 6: the batch as 2 / 4 sub-batches, each through all stages in turn (for the fused all-gather).
       //   2: full software wavefront over groups of row blocks ([1] for group j, [2]k/v for j-1, KV-attention for j-2, [4] for j-3,
-      //      [5] for j-4).  MEASURED NEGATIVE: all 73 MB of weights plus the streaming activations thrash the 126 MB L2 (DRAM reads
-      //      0.8 -> 2.0 GB per step, 0.986 -> 1.114 ms); kept as an experiment.
+      //      [5] for j-4).  An experiment, not the default: with every stage in flight the 73 MB of weights alone exceed the
+      //      50 MB L2, so the intermediates it means to keep on chip are evicted anyway.
       const char* sch_env = getenv("TP_SCHEDULE");
       const int sch = sch_env != nullptr ? atoi(sch_env) : 0;
       SegPlan plan;
@@ -1408,8 +1412,8 @@ int tp_forward_host(const void* packed, const void* x0_host, const void* xm_host
 
 #ifdef TP_GEMM_PROFILE
 // Profile builds only (libtokenpacker_b200_prof.so, not part of the public ABI): same as tp_gemm_bf16 plus a device
-// buffer [grid][16] of cycle counters: {producer wait-empty, producer total, mma wait-full, mma wait-tmem, mma total,
-// epilogue wait-accumulator, epilogue busy, -}.
+// buffer [grid][16] of cycle counters of the pair kernel: {producer wait-empty, producer total, -, -, -, epilogue warp 0: MMA
+// k-loops (ring waits included), epilogue busy, -, accumulator transposes, slab hand-offs, slab-buffer waits}.
 TP_API int tp_gemm_bf16_prof(const void* a, int64_t lda, const void* b, int64_t ldb, void* c, int64_t ldc, int64_t m, int64_t n, int64_t k,
                              const float* bias, int gelu, float alpha, long long* prof, void* stream) {
   DeviceInfo dev;

@@ -1,7 +1,7 @@
 // Kernels of the projector's backward pass that are not GEMMs: GELU forward/backward as elementwise passes, LayerNorm apply /
 // backward, window-attention backward, deterministic column sums (bias gradients), and a plain transpose (weights for the
 // dgrad GEMMs; activations only in the small-hidden wgrad fallback).  All HBM-bound, 16-byte vector accesses.
-// The GEMMs of the backward run on the forward's tcgen05 kernels: dgrad (dX = dY . W) takes a transposed copy of the weight as
+// The GEMMs of the backward run on the forward's wgmma kernels: dgrad (dX = dY . W) takes a transposed copy of the weight as
 // its K-major B operand; wgrad (dW = dY^T . X) uses the TN form, reading both activations in place as MN-major tiles.
 #pragma once
 

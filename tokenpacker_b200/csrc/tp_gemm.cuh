@@ -1,29 +1,29 @@
-// Persistent warp-specialised tcgen05 GEMMs for sm_100a with the fused epilogues the TokenPacker path needs.
+// Persistent warp-specialised wgmma GEMMs for sm_90a with the fused epilogues the TokenPacker path needs.
 //
-//   C[M,N] (bf16) = epilogue( A[M,K] (bf16, K-major) . B[N,K]^T (bf16, K-major) ),  fp32 accumulation in TMEM.
+//   C[M,N] (bf16) = epilogue( A[M,K] (bf16, K-major) . B[N,K]^T (bf16, K-major) ),  fp32 accumulation in registers.
 //
 // Every nn.Linear on the reference hot path (builder.py:59-83; MHA in/out projections builder.py:77) is an
 // instance of these kernels: activations are [rows, in] and weights are [out, in], both K-major, which is exactly the
-// operand form tcgen05.mma takes from shared memory, so no transposes exist anywhere.
+// operand form wgmma takes from shared memory, so no transposes exist anywhere.
 //
 // Two kernels share one epilogue:
-//   tp_gemm_kernel<BN>   one CTA per SM, 128 x BN tiles,  tcgen05.mma cta_group::1 (small problems, BN = 128 | 256)
-//   tp_gemm2_kernel      CTA pairs (cluster 2x1x1) on the two SMs of a TPC, 256 x 256 tiles, cta_group::2: each CTA
-//                        stages its own 128 rows of A and HALF of the B tile, so shared-memory fill traffic per FLOP
-//                        drops by a third; 4-stage mbarrier ring + double-buffered output slabs for the TMA stores.
-//                        Also the home of the TN form (MN-major operands, wgrad), multi-part A (four CLIP layers side by
-//                        side along K), grouped launches and the peer (all-gather) stores.
+//   tp_gemm_kernel<BN>   one CTA per SM, 128 x BN tiles (small problems, BN = 128 | 256)
+//   tp_gemm2_kernel      256 x 256 tiles handled by two CTAs ("a pair": CTA 2p + r computes rows r * 128 .. + 127 of the tile), each
+//                        with a 3-stage TMA ring of its 128 rows of A and the whole 256-row B tile, and double-buffered output
+//                        slabs for the TMA stores.  Also the home of the TN form (MN-major operands, wgrad), multi-part A (four
+//                        CLIP layers side by side along K), grouped launches and the peer (all-gather) stores.
 //
-// CTA = 384 threads, persistent over output tiles (default role layout):
-//   warps 0-7   epilogue: tcgen05.ld 32x32b (thread == output row), fused per-row / per-column math on the packed fp32
-//               pipe, swizzled shared-memory slabs (direct 16-byte stores in the one-CTA kernels / arbitrary row scatter)
+// CTA = 384 threads, persistent over output tiles:
+//   warps 0-7   two MMA + epilogue warpgroups, one per column half of the tile: wgmma m64nNk16 over the CTA's 128 rows (two
+//               64-row blocks, 2 x N/2 fp32 accumulators per thread), then the epilogue on the same registers: each warp turns its
+//               fragments into thread == output row form through a 2 KiB shared-memory transpose (32 columns at a time), fused
+//               per-row / per-column math, swizzled shared-memory slabs (16-byte stores) or direct 16-byte global stores
 //   warps 8, 9  store warps of the pair kernel (one per column half): wait for a finished slab on an mbarrier, issue its TMA
 //               store(s), hand the buffer back, and — for GEMMs that other GEMMs of the same launch depend on — publish each
-//               finished tile to a global counter.  The epilogue warps never wait for a store.  Warp 9 also allocates TMEM
-//               (2 accumulator buffers: the epilogue of tile i overlaps tile i+1's MMAs)
+//               finished tile to a global counter.  The epilogue warps never wait for a store.
 //   warp 10     TMA producer   (warp-uniform loop, elect.sync around the issue): cp.async.bulk.tensor boxes, 128B swizzle, mbarrier
 //               ring; spins on the producer GEMM's tile counter before the first load of a dependent tile
-//   warp 11     MMA issuer     (leader CTA only in pair mode): fp32 accumulators in TMEM
+//   (warps 8-11 run with 72 registers a thread, setmaxnreg, so that the accumulator warpgroups can hold 216)
 //
 // Fused epilogue (all optional, selected at run time, warp-uniform branches):
 //   v = acc
@@ -71,7 +71,7 @@ struct GemmEpilogue {
 };
 
 #ifndef TP_EPI_SUB_PAIRS
-#define TP_EPI_SUB_PAIRS 8      // 4 / 8 / 16 measured: 8 = most interleaving that still fits the register budget without spills
+#define TP_EPI_SUB_PAIRS 8      // column pairs per warp-uniform epilogue block: more independent chains for the scheduler, more registers
 #endif
 
 #ifdef TP_GEMM_PROFILE
@@ -86,27 +86,119 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;     // 64 bf16 = 128 bytes = one swizzle-128B row
 constexpr int kUmmaK = 16;
 constexpr int kGemmThreads = 384;
-// Warp roles.  The warp scheduler favours higher warp ids when several warps of an SM sub-partition are eligible, and
-// the single-lane TMA / MMA warps must never lose an issue slot to the (instruction-heavy) epilogue warps: they get
-// the HIGHEST ids.  Epilogue warp w reads TMEM lanes 32*(w % 4)..+31 (hardware restriction), so 8 epilogue warps =
-// 4 lane quarters x 2 column halves.
+// Warp roles: warps 0-7 are the two MMA + epilogue warpgroups (warpgroup = column half of the tile, warp % 4 = "quarter": the
+// 16 + 16 rows of each 64-row block its wgmma fragments hold), warps 8-11 the producer / store warpgroup.
 constexpr int kEpiWarp0 = 0;
 constexpr int kTmaWarp = 10;
-constexpr int kMmaWarp = 11;
-constexpr int kAllocWarp = 9;
-constexpr int kStoreWarp0 = 8;      // pair kernel: warps 8 and 9 issue the TMA stores of column half 0 / 1 (role layout 1 only)
+constexpr int kStoreWarp0 = 8;      // pair kernel: warps 8 and 9 issue the TMA stores of column half 0 / 1
 constexpr int kNumEpiWarps = 8;
 constexpr int kEpiThreads = kNumEpiWarps * 32;
 constexpr int kEpiBarrierId = 1;
+constexpr uint32_t kMmaRegs = 216;  // setmaxnreg: 256 x 216 + 128 x 72 <= 64 K registers of an SM
+constexpr uint32_t kAuxRegs = 72;
+constexpr int kScratchBytesPerWarp = 32 * 16 * 4;     // accumulator transpose: 32 rows x 16 fp32 columns
+constexpr int kScratchBytes = kNumEpiWarps * kScratchBytesPerWarp;
+
+// Tile row of epilogue thread (quarter, lane): the rows whose wgmma fragments warp `quarter` of a warpgroup holds — 16 of each
+// 64-row block — so the fragment -> row transpose never leaves the warp.  Windows of 4 or 16 consecutive rows stay inside 16
+// consecutive lanes.
+__device__ __forceinline__ int epi_row(int quarter, uint32_t lane) {
+  return 16 * quarter + static_cast<int>(lane & 15u) + 64 * static_cast<int>(lane >> 4);
+}
+
+// 32 accumulator columns [32 chunk, +32) of this warp's 32 rows (epi_row order) into r: each thread gets its own row.  The two
+// 64-row blocks' fragments go through the warp's scratch, 16 columns at a time, XOR-swizzled so that both the 8-byte fragment
+// stores and the 16-byte row loads are free of bank conflicts.  `chunk` must be a compile-time constant after unrolling.
+__device__ __forceinline__ uint32_t scratch_swz(uint32_t row) { return (((row >> 1) & 1u) << 1) | ((row >> 2) & 1u); }
+
+template <int kAccN>
+__device__ __forceinline__ void acc_chunk(const float (&acc)[2][kAccN], int chunk, uint32_t scratch, uint32_t (&r)[32]) {
+  const uint32_t lane = lane_id();
+  const uint32_t g = lane >> 2, q = lane & 3u;
+#pragma unroll
+  for (int t = 0; t < 2; ++t) {
+    __syncwarp();                                      // the previous reads of the scratch are done
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+          const int i = (chunk * 4 + t * 2 + jj) * 4 + 2 * h;
+          const uint32_t row = g + 8u * h + 16u * mb;
+          const uint32_t unit = ((2u * jj) + (q >> 1)) ^ scratch_swz(row);
+          sts_f2(scratch + row * 64u + unit * 16u + (q & 1u) * 8u, acc[mb][i], acc[mb][i + 1]);
+        }
+    __syncwarp();
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const float4 v = lds_f4_ordered(scratch + lane * 64u + ((static_cast<uint32_t>(u) ^ scratch_swz(lane)) * 16u));
+      r[16 * t + 4 * u + 0] = __float_as_uint(v.x);
+      r[16 * t + 4 * u + 1] = __float_as_uint(v.y);
+      r[16 * t + 4 * u + 2] = __float_as_uint(v.z);
+      r[16 * t + 4 * u + 3] = __float_as_uint(v.w);
+    }
+  }
+}
+
+// One warpgroup's MMAs for a tile: the CTA's 128 rows of A (two 64-row blocks) x kN columns of B starting `b_off` bytes into
+// the stage's B tile, over n_kb k-blocks of the ring.  A stage is released (one arrive per warp on empty_bar) once the wgmmas
+// reading it have retired; one k-block of wgmmas stays in flight while the next one is issued.
+template <int kN, int kTransA, int kTransB>
+__device__ __forceinline__ void mma_tile(float (&acc)[2][kN / 2], const uint8_t* smem, int stage_bytes, int a_bytes, int b_off,
+                                         uint64_t* full_bar, uint64_t* empty_bar, int n_stages, int& stage, uint32_t& phase, int n_kb) {
+  static_assert(kN == 64 || kN == 128, "wgmma N");
+  int prev = -1;
+  for (int kb = 0; kb < n_kb; ++kb) {
+    mbar_wait(&full_bar[stage], phase);         // TMA bytes have landed
+    const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+    const uint32_t sb = sa + static_cast<uint32_t>(a_bytes + b_off);
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) fence_regs(acc[mb]);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < kBlockK / kUmmaK; ++k) {
+      // K-major: advance 16 elements = 32 bytes along the 128-byte swizzle row (+2 in the address field);
+      // MN-major: one k16 step = two 8-row K groups = 2 KiB (+128); 64-row blocks of A and 64-wide MN atoms are 8 KiB apart
+      const uint64_t db = kTransB ? make_smem_desc_mnmajor_sw128(sb, 8192) + static_cast<uint64_t>(k * 128)
+                                  : make_smem_desc_kmajor_sw128(sb) + static_cast<uint64_t>(k * 2);
+      const uint32_t accumulate = static_cast<uint32_t>((kb | k) != 0);
+#pragma unroll
+      for (int mb = 0; mb < 2; ++mb) {
+        const uint32_t sam = sa + static_cast<uint32_t>(mb * 8192);
+        const uint64_t da = kTransA ? make_smem_desc_mnmajor_sw128(sam, 8192) + static_cast<uint64_t>(k * 128)
+                                    : make_smem_desc_kmajor_sw128(sam) + static_cast<uint64_t>(k * 2);
+        if constexpr (kN == 128) wgmma_m64n128<kTransA, kTransB>(acc[mb], da, db, accumulate);
+        else wgmma_m64n64<kTransA, kTransB>(acc[mb], da, db, accumulate);
+      }
+    }
+    wgmma_commit();
+#pragma unroll
+    for (int mb = 0; mb < 2; ++mb) fence_regs(acc[mb]);
+    wgmma_wait<1>();                                   // the previous k-block's wgmmas have retired
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane_id() == 0) mbar_arrive(&empty_bar[prev]);
+    }
+    prev = stage;
+    if (++stage == n_stages) { stage = 0; phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int mb = 0; mb < 2; ++mb) fence_regs(acc[mb]);
+  if (prev >= 0) {
+    __syncwarp();
+    if (lane_id() == 0) mbar_arrive(&empty_bar[prev]);
+  }
+}
 
 // ------------------------------------------------------------------------------------------------
-// Shared epilogue for one 128-row x kTileN-column accumulator tile held in this CTA's TMEM.
-//   tmem_acc : TMEM address of the accumulator buffer (column offset applied, lane 0)
-//   row      : global output row of this thread (lane of TMEM == row inside the tile)
+// Shared epilogue for one 128-row x kTileN-column accumulator tile held in the registers of the CTA's two MMA warpgroups.
+//   acc      : this warpgroup's (= column half's) wgmma accumulators
+//   scratch  : shared address of this warp's transpose scratch (kScratchBytesPerWarp)
+//   row      : global output row of this thread (tile row epi_row(quarter, lane))
 //   col_tile0: global column of the tile's first column
 //   s_col    : shared staging for this tile's col_a / col_b slices, [2][kTileN] floats (already filled + synced)
-// `release()` is invoked as soon as the last tcgen05.ld of this warp has landed in registers, so the MMA warp gets
-// the TMEM buffer back before the math / stores of the final chunk.
 // ------------------------------------------------------------------------------------------------
 // Output staging for TMA stores: each column half of the tile (4 warps) owns two 16 KiB buffers holding a 128-row x 64-col
 // slab in the 128B-swizzled layout; a slab is written with conflict-free 16-byte st.shared, then ONE thread hands it
@@ -131,8 +223,9 @@ struct OutStage {
   bool swizzle;              // slab rows in the TMA swizzle of the row width (false: plain rows, for C maps built without swizzle)
 };
 // Output slab = 128 rows x kSlabCols columns of bf16, in the TMA swizzle of that row width (64 columns: 128-byte rows,
-// SWIZZLE_128B; 32 columns: 64-byte rows, SWIZZLE_64B).  The narrow form halves the staging memory, which buys two more
-// stages of the operand ring (-DTP_SLAB_COLS=32 -DTP_PAIR_STAGES=6): the ring depth is what hides operand-fetch latency.
+// SWIZZLE_128B; 32 columns: 64-byte rows, SWIZZLE_64B).  The narrow form halves the staging memory (32 KiB freed): not enough
+// for a fourth 48 KiB ring stage of the pair kernel, so it only matters with -DTP_OUT_BUFS=1 -DTP_SLAB_COLS=32 -DTP_PAIR_STAGES=4
+// (which gives up the dual pre-activation output of the training forward).
 #ifndef TP_SLAB_COLS
 #define TP_SLAB_COLS 64
 #endif
@@ -156,7 +249,7 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
   const float2* st = reinterpret_cast<const float2*>(stats) + row * slots;
   float t1 = 0.f, m2 = 0.f;
   for (int i = 0; i < slots; ++i) t1 = __fadd_rn(t1, st[i].x);
-  const float inv_slots = __frcp_rn(static_cast<float>(slots));
+  const float inv_slots = rcp_rn_normal(static_cast<float>(slots));      // slots in [1, 64], inv_dim in [2^-13, 1]: call-free
   mu = __fmul_rn(t1, inv_slots);
   float between = 0.f;
   for (int i = 0; i < slots; ++i) {
@@ -165,13 +258,13 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
     between = fmaf(d, d, between);
     m2 = __fadd_rn(m2, v.y);
   }
-  const float var = __fmul_rn(fmaf(between, __fmul_rn(inv_slots, __frcp_rn(inv_dim)), m2), inv_dim);
+  const float var = __fmul_rn(fmaf(between, __fmul_rn(inv_slots, rcp_rn_normal(inv_dim)), m2), inv_dim);
   rstd = rsqrtf(__fadd_rn(var, eps));
 }
 
-template <int kTileN, typename ReleaseFn>
-__device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int N, uint32_t tmem_acc, int row, int col_tile0,
-                                              int quarter, int half, const float* s_col, const OutStage& out, ReleaseFn release,
+template <int kTileN>
+__device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int N, const float (&acc)[2][kTileN / 4], uint32_t scratch,
+                                              int row, int col_tile0, int quarter, int half, const float* s_col, const OutStage& out,
                                               [[maybe_unused]] long long* pc = nullptr, long long c_extra = 0) {
   constexpr int kColsPerWarp = kTileN / 2;
   constexpr int kChunks = kColsPerWarp / 32;
@@ -193,7 +286,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
   }
   __nv_bfloat16* c_row = ep.c + dst_row * ep.ldc;
   float* c_row32 = reinterpret_cast<float*>(ep.c) + c_extra + dst_row * ep.ldc;     // out_f32 only (c_extra: split-K slice)
-  const uint32_t taddr = tmem_acc + (static_cast<uint32_t>(quarter * 32) << 16) + static_cast<uint32_t>(half * kColsPerWarp);
   const uint32_t sa_addr = smem_u32(s_col + half * kColsPerWarp), sb_addr = smem_u32(s_col + kTileN + half * kColsPerWarp);
   const uint32_t out_addr = out.buf != nullptr ? smem_u32(out.buf) : 0u;
 
@@ -201,17 +293,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
   const bool do_stats = ep.stats_out != nullptr;
   const bool scale = ep.alpha != 1.0f;
   const uint64_t rstd2 = pk2(rstd), nmu2 = pk2(-mu), alpha2 = pk2(ep.alpha);
-  uint32_t r[2][32];
-  tmem_ld_32x32b_x32(taddr, r[0]);
+  uint32_t r[32];
 #pragma unroll
   for (int chunk = 0; chunk < kChunks; ++chunk) {
     {
       TP_PROF_T0();
-      tmem_ld_wait();
+      acc_chunk(acc, chunk, scratch, r);
       TP_PROF_ADD(pc[0]);
     }
-    if (chunk + 1 < kChunks) tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>((chunk + 1) * 32), r[(chunk + 1) & 1]);
-    else release();                                   // every TMEM read of this warp has landed in registers
     const int col0 = col_tile0 + half * kColsPerWarp + chunk * 32;
     // dual output: every 64-column slab exists twice — pre-activation (even slab number, buffer 0) and activation (odd, buffer 1)
     const bool dual = ep.dual != 0 && out.buf != nullptr;
@@ -229,17 +318,17 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
       // kSubPairs packed pairs (2 columns each) go through every step together: each run-time option is ONE warp-uniform branch
       // around a basic block of kSubPairs independent dependency chains for the scheduler to interleave.
       constexpr int kSubPairs = TP_EPI_SUB_PAIRS;
-      const int rloc = quarter * 32 + static_cast<int>(lane_id());
+      const int rloc = epi_row(quarter, lane_id());
 #pragma unroll
       for (int sub = 0; sub < 16 / kSubPairs; ++sub) {
         const int lc = chunk * 32 + sub * kSubPairs * 2;             // first column of this sub-block inside the warp's slice
         uint64_t v[kSubPairs];
 #pragma unroll
         for (int j = 0; j < kSubPairs; ++j)
-          v[j] = pk2(__uint_as_float(r[chunk & 1][sub * kSubPairs * 2 + 2 * j]), __uint_as_float(r[chunk & 1][sub * kSubPairs * 2 + 2 * j + 1]));
+          v[j] = pk2(__uint_as_float(r[sub * kSubPairs * 2 + 2 * j]), __uint_as_float(r[sub * kSubPairs * 2 + 2 * j + 1]));
         const uint32_t sb4 = sb_addr + static_cast<uint32_t>(lc) * 4u;
-        if (ln_fold) {     // v = fma(rstd, fma(-mu, col_a, v), col_b): explicit fmas — ptxas contracts adjacent mul.f32x2 / add.f32x2
-          const uint32_t sa4 = sa_addr + static_cast<uint32_t>(lc) * 4u;    // pairs when it sees them, and not in every instantiation alike
+        if (ln_fold) {     // v = fma(rstd, fma(-mu, col_a, v), col_b): explicit fmas, the same in every instantiation
+          const uint32_t sa4 = sa_addr + static_cast<uint32_t>(lc) * 4u;
 #pragma unroll
           for (int q = 0; q < kSubPairs / 2; ++q) {
             const float4 a = lds_f4(sa4 + q * 16), b = lds_f4(sb4 + q * 16);
@@ -357,8 +446,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
 //              by 1/sqrt 128), softmax over the s*s consecutive lanes of the window (warp shuffles)  -> p stays in a register
 //     phase V: v' = y_v . (gamma_v W_iv)^T                     -> epilogue: folded LayerNorm, p * v', halving exchange over the window's
 //              lanes, store the window's 128 context channels of the head
-//   The two phases use the two TMEM accumulator buffers alternately, so the MMAs of phase V run under the score epilogue and the
-//   next tile's phase K under the P.V epilogue: the tensor pipe sees the same back-to-back 256-wide k-loops as a plain GEMM.
+//   Both phases use the same accumulator registers one after the other; the producer keeps the ring full in the meantime.
 //   Thread == key row; column half (warps 0-3 / 4-7) == head of the pair.  k' and v' never exist in memory (fp32, unrounded, in
 //   registers): the [R,1024] x 2 round trip through HBM and the separate attention kernel are gone.
 // ------------------------------------------------------------------------------------------------
@@ -389,9 +477,8 @@ __device__ __forceinline__ float bf16x2_get(const uint4& v, int i) {      // i i
 }
 
 // Phase K epilogue: returns this row's softmax weight p for head `head`.  s_vec: [wsum | cst][256] of the tile's two heads.
-template <typename ReleaseFn>
-__device__ __forceinline__ float attn_scores(const AttnParams& at, int M, uint32_t tmem_acc, int row, int head, int quarter, int half,
-                                             const float* s_vec, ReleaseFn release) {
+__device__ __forceinline__ float attn_scores(const AttnParams& at, int M, const float (&acc)[2][64], uint32_t scratch, int row, int head,
+                                             int half, const float* s_vec) {
   const int W = at.s * at.s;
   const bool row_ok = row < M;
   float mu = 0.f, rstd = 0.f;
@@ -399,39 +486,34 @@ __device__ __forceinline__ float attn_scores(const AttnParams& at, int M, uint32
   const long long window = row / W;
   const float* wsum = s_vec + half * 128;
   const float* cst = s_vec + 256 + half * 128;
-  const uint32_t taddr = tmem_acc + (static_cast<uint32_t>(quarter * 32) << 16) + static_cast<uint32_t>(half * 128);
   const uint4* qrow = reinterpret_cast<const uint4*>(at.qp + window * 1024 + head * 128);
-  uint32_t r[2][32];
-  tmem_ld_32x32b_x32(taddr, r[0]);
+  uint32_t r[32];
   float score = 0.f;
 #pragma unroll
   for (int chunk = 0; chunk < 4; ++chunk) {
-    tmem_ld_wait();
-    if (chunk + 1 < 4) tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>((chunk + 1) * 32), r[(chunk + 1) & 1]);
-    else release();                                   // every TMEM read of this warp has landed in registers
+    acc_chunk(acc, chunk, scratch, r);
     uint4 q4[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) q4[i] = row_ok ? __ldg(qrow + chunk * 4 + i) : make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
     for (int c = 0; c < 32; ++c) {
-      const float kf = fmaf(rstd, fmaf(-mu, wsum[chunk * 32 + c], __uint_as_float(r[chunk & 1][c])), cst[chunk * 32 + c]);
+      const float kf = fmaf(rstd, fmaf(-mu, wsum[chunk * 32 + c], __uint_as_float(r[c])), cst[chunk * 32 + c]);
       score = fmaf(bf16x2_get(q4[c >> 3], c & 7), kf, score);
     }
   }
-  // softmax over the W keys of my window = W consecutive lanes (W divides 32, windows never straddle a warp)
+  // softmax over the W keys of my window = W consecutive lanes (W divides 16: windows never straddle a 16-lane half, see epi_row)
   float mx = score;
   for (int off = 1; off < W; off <<= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
   const float e = __expf(score - mx);
   float den = e;
   for (int off = 1; off < W; off <<= 1) den += __shfl_xor_sync(0xffffffffu, den, off);
-  return e * (1.0f / den);
+  return e * rcp_rn_normal(den);                    // den in [1, 16]: the correctly rounded 1 / den, without a call
 }
 
 // Phase V epilogue: ctx = sum over the window's lanes of p * v'.  Halving exchange: after log2(W) steps each lane holds 32 / W
 // channels of the chunk.
-template <typename ReleaseFn>
-__device__ __forceinline__ void attn_pv(const AttnParams& at, int M, uint32_t tmem_acc, int row, int head, int quarter, int half, float p,
-                                        const float* s_vec, ReleaseFn release) {
+__device__ __forceinline__ void attn_pv(const AttnParams& at, int M, const float (&acc)[2][64], uint32_t scratch, int row, int head, int half,
+                                        float p, const float* s_vec) {
   const int W = at.s * at.s;
   const bool row_ok = row < M;
   const uint32_t lane = lane_id();
@@ -440,18 +522,14 @@ __device__ __forceinline__ void attn_pv(const AttnParams& at, int M, uint32_t tm
   const long long window = row / W;
   const float* wsum = s_vec + half * 128;
   const float* cst = s_vec + 256 + half * 128;
-  const uint32_t taddr = tmem_acc + (static_cast<uint32_t>(quarter * 32) << 16) + static_cast<uint32_t>(half * 128);
-  uint32_t r[2][32];
-  tmem_ld_32x32b_x32(taddr, r[0]);
+  uint32_t r[32];
 #pragma unroll
   for (int chunk = 0; chunk < 4; ++chunk) {
-    tmem_ld_wait();
-    if (chunk + 1 < 4) tmem_ld_32x32b_x32(taddr + static_cast<uint32_t>((chunk + 1) * 32), r[(chunk + 1) & 1]);
-    else release();
+    acc_chunk(acc, chunk, scratch, r);
     float v[32];
 #pragma unroll
     for (int c = 0; c < 32; ++c)
-      v[c] = p * fmaf(rstd, fmaf(-mu, wsum[chunk * 32 + c], __uint_as_float(r[chunk & 1][c])), cst[chunk * 32 + c]);
+      v[c] = p * fmaf(rstd, fmaf(-mu, wsum[chunk * 32 + c], __uint_as_float(r[c])), cst[chunk * 32 + c]);
     int first = 0;                                    // my live values cover channels [first, first + 32 >> steps) of the chunk
 #pragma unroll
     for (int step = 0; step < 4; ++step) {
@@ -498,14 +576,14 @@ __device__ __forceinline__ void stage_col_vectors(const GemmEpilogue& ep, int N,
 // ================================================================================================
 template <int kBlockN>
 struct GemmConfig {
-  static constexpr int kStages = (kBlockN == 256) ? 4 : 6;
+  static constexpr int kStages = 4;
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = kBlockN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = 2 * kBlockN;  // double-buffered accumulator
-  static constexpr int kColStageBytes = 2 * 2 * kBlockN * 4;   // [2 buffers][col_a | col_b][kBlockN] floats
-  static constexpr int kBarrierBytes = (2 * kStages + 4) * 8 + 16;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kColStageBytes + kBarrierBytes + 1024;  // +1024: manual alignment
+  static constexpr int kColStageBytes = 2 * kBlockN * 4;   // [col_a | col_b][kBlockN] floats
+  static constexpr int kBarrierBytes = 2 * kStages * 8;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kScratchBytes + kColStageBytes + kBarrierBytes + 1024;  // +1024: manual alignment
+  static_assert(kSmemBytes <= 232448, "shared memory budget of an sm_90 SM (227 KiB)");
 };
 
 template <int kBlockN>
@@ -514,16 +592,15 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                int a_seg_rows, GemmEpilogue ep) {
   using Cfg = GemmConfig<kBlockN>;
   constexpr int kStages = Cfg::kStages;
+  constexpr int kN = kBlockN / 2;                  // columns per warpgroup
   static_assert(kBlockN == 128 || kBlockN == 256, "BLOCK_N");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  float* s_col_base = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes + Cfg::kColStageBytes);
+  uint8_t* s_scratch = smem + kStages * Cfg::kStageBytes;
+  float* s_col = reinterpret_cast<float*>(s_scratch + kScratchBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_scratch + kScratchBytes + Cfg::kColStageBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full_bar = empty_bar + kStages;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
 
   const int warp_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const uint32_t lane = lane_id();
@@ -536,29 +613,20 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   if (warp_idx == kTmaWarp && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
-  } else if (warp_idx == kMmaWarp && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);
-      mbar_init(&tmem_empty_bar[i], kNumEpiWarps);
+      mbar_init(&empty_bar[i], kNumEpiWarps);      // one arrive per MMA warp
     }
     fence_barrier_init();
-  } else if (warp_idx == kAllocWarp) {
-    tmem_alloc<Cfg::kTmemCols>(tmem_base_smem);
   }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
   grid_dependency_wait();                  // PDL: the prologue above overlapped the previous kernel's tail
   grid_launch_dependents();
 
-  if (warp_idx == kTmaWarp) {
-    // ======================================= TMA producer =======================================
-    if (lane == 0) {
+  if (warp_idx >= kNumEpiWarps) {
+    setmaxnreg_dec<kAuxRegs>();
+    if (warp_idx == kTmaWarp && lane == 0) {
+      // ======================================= TMA producer =======================================
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -586,75 +654,32 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       }
     }
     __syncwarp();
-  } else if (warp_idx == kMmaWarp) {
-    // ======================================= MMA issuer =========================================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16_f32(kBlockM, kBlockN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u);   // epilogue has drained this accumulator buffer
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(acc * kBlockN);
-        for (int kb = 0; kb < num_k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);                // TMA bytes have landed
-          tcgen05_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint64_t desc_a = make_smem_desc_kmajor_sw128(sa);
-          const uint64_t desc_b = make_smem_desc_kmajor_sw128(sa + Cfg::kABytes);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            // advance 16 elements = 32 bytes along K inside the 128-byte swizzle row: +2 in the (addr >> 4) field
-            umma_bf16(tmem_d, desc_a + static_cast<uint64_t>(k * 2), desc_b + static_cast<uint64_t>(k * 2), idesc,
-                      static_cast<uint32_t>((kb | k) != 0));
-          }
-          umma_commit(&empty_bar[stage]);                    // smem slot reusable once these MMAs retire
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(&tmem_full_bar[acc]);                    // accumulator complete -> epilogue
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-    }
-    __syncwarp();
-  } else if (warp_idx >= kEpiWarp0 && warp_idx < kEpiWarp0 + kNumEpiWarps) {
-    // ======================================= epilogue ===========================================
+  } else {
+    // ======================================= MMA + epilogue (warpgroup = column half) =============
+    setmaxnreg_inc<kMmaRegs>();
     const int e = warp_idx - kEpiWarp0;
-    const int quarter = warp_idx & 3;            // TMEM lane quarter this warp may access
-    const int half = e >> 2;                     // which half of the tile's columns
+    const int quarter = warp_idx & 3;
+    const int half = e >> 2;
     const int epi_tid = e * 32 + static_cast<int>(lane);
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    const uint32_t scratch = smem_u32(s_scratch + e * kScratchBytesPerWarp);
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[2][kN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int m_blk = tile / num_n_blocks;
       const int n_blk = tile - m_blk * num_n_blocks;
-      float* s_col = s_col_base + acc * 2 * kBlockN;
-      stage_col_vectors<kBlockN>(ep, N, n_blk * kBlockN, s_col, epi_tid);
-      mbar_wait(&tmem_full_bar[acc], acc_phase);
-      tcgen05_fence_after();
-      uint64_t* release_bar = &tmem_empty_bar[acc];
+      stage_col_vectors<kBlockN>(ep, N, n_blk * kBlockN, s_col, epi_tid, true);
+      mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, half * kN * kBlockK * 2, full_bar, empty_bar, kStages, stage, phase,
+                         num_k_blocks);
       const OutStage no_stage{nullptr, nullptr, nullptr, 1, 0u, true};
-      epilogue_tile<kBlockN>(ep, M, N, tmem_base + static_cast<uint32_t>(acc * kBlockN),
-                             m_blk * kBlockM + quarter * 32 + static_cast<int>(lane), n_blk * kBlockN, quarter, half, s_col, no_stage, [&]() {
-                               tcgen05_fence_before();
-                               __syncwarp();
-                               if (lane == 0) mbar_arrive(release_bar);
-                             });
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+      epilogue_tile<kBlockN>(ep, M, N, acc, scratch, m_blk * kBlockM + epi_row(quarter, lane), n_blk * kBlockN, quarter, half, s_col,
+                             no_stage);
     }
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp_idx == kAllocWarp) {
-    tcgen05_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
   }
 }
 
 // ================================================================================================
-// CTA-pair kernel: 256 x 256 tiles, cta_group::2, GROUPED: one launch runs up to kMaxGroup independent GEMM problems
+// Pair kernel: 256 x 256 tiles (two CTAs of 128 rows each), GROUPED: one launch runs up to kMaxGroup independent GEMM problems
 // (e.g. k_proj_1.2 | v_proj_1.2 | q_proj_1, which share no data but would each leave the machine with a partial last
 // wave and pay launch + prologue + drain on their own).  Tiles are numbered across the problems of the group; every warp
 // role walks the same sequence.
@@ -663,27 +688,23 @@ struct Gemm2Config {
   static constexpr int kTileM = 256;
   static constexpr int kTileN = 256;
 #ifndef TP_PAIR_STAGES
-#define TP_PAIR_STAGES 5
+#define TP_PAIR_STAGES 3
 #endif
 #ifndef TP_OUT_BUFS
-#define TP_OUT_BUFS ((TP_PAIR_STAGES <= 5 || TP_SLAB_COLS == 32) ? 2 : 1)
+#define TP_OUT_BUFS 2
 #endif
-  // Ring depth is what hides the operand-fetch latency (measured on the configs[1] step, same box: 4 / 5 / 6 stages = 1.001 /
-  // 0.967 / 0.973 ms); since the store warps took the TMA stores off the epilogue warps' path one staging slab per column half is
-  // enough, which is what pays for the fifth stage.
   static constexpr int kStages = TP_PAIR_STAGES;
   static constexpr int kOutBufs = TP_OUT_BUFS;                   // staging buffers per column half (1 or 2)
   static constexpr int kABytes = kBlockM * kBlockK * 2;          // this CTA's 128 rows of A
-  static constexpr int kBBytes = (kTileN / 2) * kBlockK * 2;     // this CTA's half of the B tile
-  static constexpr int kStageBytes = kABytes + kBBytes;          // 32 KiB
-  static constexpr int kTmemCols = 2 * kTileN;
+  static constexpr int kBBytes = kTileN * kBlockK * 2;           // the whole B tile
+  static constexpr int kStageBytes = kABytes + kBBytes;          // 48 KiB
   static constexpr int kOutBytes = 2 * kOutBufs * kOutSlabBytes; // [2 column halves][kOutBufs] output slabs for TMA stores
   static constexpr int kColStageBytes = 2 * kTileN * 4;          // [col_a | col_b][kTileN] floats, ONE buffer (barrier before it is rewritten)
-  static constexpr int kBarrierBytes = (2 * kStages + 4 + 4 * kOutBufs) * 8 + 16;   // ring + accumulators + slab full/empty per half
-  // 5 stages x 32 KiB + 4 x 16 KiB slabs + 2 KiB + barriers = 226.2 KiB of the 227 KiB an SM offers: the dynamic shared memory is
-  // declared 1024-byte aligned (no alignment slack), and the per-column vectors are single-buffered
-  static constexpr int kSmemBytes = kStages * kStageBytes + kOutBytes + kColStageBytes + kBarrierBytes;
-  static_assert(kSmemBytes <= 232448, "shared memory budget of an sm_100 SM (227 KiB)");
+  static constexpr int kBarrierBytes = (2 * kStages + 4 * kOutBufs) * 8;   // ring + slab full/empty per half
+  // 3 stages x 48 KiB + 4 x 16 KiB slabs + 16 KiB transpose scratch + 2 KiB + barriers = 226.1 KiB of the 227 KiB an SM offers: the
+  // dynamic shared memory is declared 1024-byte aligned (no alignment slack), and the per-column vectors are single-buffered
+  static constexpr int kSmemBytes = kStages * kStageBytes + kOutBytes + kScratchBytes + kColStageBytes + kBarrierBytes;
+  static_assert(kSmemBytes <= 232448, "shared memory budget of an sm_90 SM (227 KiB)");
 };
 
 constexpr int kMaxGroup = 8;
@@ -722,7 +743,7 @@ struct GemmProblem {
   long long c_split_stride;   // floats between consecutive split slices of C
   // Dependencies between GEMMs of ONE launch (a chain of linears runs as a single persistent kernel: no ramp / drain / partial
   // last wave per layer).  Tiles are numbered problem after problem and every CTA pair walks its tiles in increasing order, so a
-  // tile only ever waits for lower-numbered tiles: no deadlock as long as all pairs are co-resident (grid <= 74 pairs).
+  // tile only ever waits for lower-numbered tiles: no deadlock as long as all CTAs are co-resident (grid <= one CTA per SM).
   int* done_counter;     // != nullptr: [ceil(M/256)] tile counter of THIS problem's output row blocks, +1 per (CTA, column half)
                          //             once that part of a tile is in global memory (bumped by the store warps)
   const int* dep_counter;// != nullptr: the A operand's row block m_blk is ready when dep_counter[m_blk >> dep_shift] >= dep_target
@@ -815,28 +836,26 @@ __device__ __forceinline__ TileRef decode_tile(const GemmGroup& g, int tile, int
   return t;
 }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGemmThreads, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ PeerStores peers) {
   using Cfg = Gemm2Config;
   constexpr int kStages = Cfg::kStages;
   constexpr int kTileN = Cfg::kTileN;
+  constexpr int kN = kTileN / 2;                                // columns per warpgroup
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];     // 1 KiB aligned: swizzle atoms of the operand tiles and output slabs
   uint8_t* smem = smem_raw;
   uint8_t* s_out = smem + kStages * Cfg::kStageBytes;                                  // 1 KiB aligned (swizzle atoms)
-  float* s_col_base = reinterpret_cast<float*>(s_out + Cfg::kOutBytes);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_out + Cfg::kOutBytes + Cfg::kColStageBytes);
+  uint8_t* s_scratch = s_out + Cfg::kOutBytes;
+  float* s_col_base = reinterpret_cast<float*>(s_scratch + kScratchBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_scratch + kScratchBytes + Cfg::kColStageBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full_bar = empty_bar + kStages;
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;
-  uint64_t* slab_full_bar = tmem_empty_bar + 2;                 // [2 halves][kOutBufs]
+  uint64_t* slab_full_bar = empty_bar + kStages;                // [2 halves][kOutBufs]
   uint64_t* slab_empty_bar = slab_full_bar + 2 * Cfg::kOutBufs; // [2 halves][kOutBufs]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(slab_empty_bar + 2 * Cfg::kOutBufs);
 
   const int warp_idx = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const uint32_t lane = lane_id();
-  const uint32_t cta_rank = cluster_ctarank();
-  const bool is_leader = cta_rank == 0;
+  const uint32_t cta_rank = blockIdx.x & 1u;                   // which 128 rows of the pair's 256-row tile this CTA computes
   const int num_tiles = grp.total_tiles;
   const int pair_idx = static_cast<int>(blockIdx.x >> 1);
   const int num_pairs = static_cast<int>(gridDim.x >> 1);
@@ -852,259 +871,34 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       }
       if (grp.p[i].use_tma_store) tma_prefetch_desc(&grp.p[i].tmap_c);
     }
-  } else if (warp_idx == kMmaWarp && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 2);          // one arrival per CTA's producer (the leader's carries the expected bytes of both)
-      mbar_init(&empty_bar[i], 1);         // multicast tcgen05.commit from the leader
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full_bar[i], 1);                   // multicast tcgen05.commit from the leader
-      mbar_init(&tmem_empty_bar[i], 2 * kNumEpiWarps);   // epilogue warps of BOTH CTAs (waited on in the leader only)
+      mbar_init(&full_bar[i], 1);                        // the producer's expect-tx arrive
+      mbar_init(&empty_bar[i], kNumEpiWarps);            // one arrive per MMA warp
     }
     for (int i = 0; i < 2 * Cfg::kOutBufs; ++i) {
       mbar_init(&slab_full_bar[i], kNumEpiWarps / 2);    // one arrive per epilogue warp of the column half
       mbar_init(&slab_empty_bar[i], 1);                  // the half's store warp
     }
     fence_barrier_init();
-  } else if (warp_idx == kAllocWarp) {
-    tmem_alloc_pair<Cfg::kTmemCols>(tmem_base_smem);
   }
-  tcgen05_fence_before();
-  cluster_sync_all();                      // barriers of both CTAs initialised before any remote arrive / multicast commit
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
+  __syncthreads();
   // Programmatic dependent launch: everything above overlapped the tail of the previous kernel on the stream; from here
   // on we read what it wrote.  (No-op when the launch carries no PDL attribute.)
   grid_dependency_wait();
   grid_launch_dependents();                // the next kernel's CTAs may take over SMs as ours exit (they block in their own wait)
-
-  if (warp_idx == kTmaWarp) {
-    // ======================================= TMA producer (both CTAs) ============================
-    // Whole warp runs the loop (uniform control flow); one elected lane issues the arrive + TMA instructions.
-    int stage = 0, cursor = 0;
-    uint32_t phase = 0;
-    [[maybe_unused]] long long w_empty = 0;
-    [[maybe_unused]] const long long t_begin = clock64();
-    for (int tile = pair_idx; tile < num_tiles; tile += num_pairs) {
-      const TileRef t = decode_tile(grp, tile, cursor);
-      const GemmProblem& pr = *t.pr;
-      const int row0 = t.m_blk * Cfg::kTileM + static_cast<int>(cta_rank) * kBlockM;          // my 128 rows of A
-      const int brow0 = t.n_blk * kTileN + static_cast<int>(cta_rank) * (kTileN / 2);        // my half of the B tile
-      // segmented A (3-D map, 64-row boxes): global row g -> (segment g / seg_rows, row g % seg_rows); hoisted per tile
-      if (pr.dep_counter != nullptr) {
-        // A's row block is written by an earlier problem of this launch: wait until all its tiles have been published (acquire),
-        // then order the TMA (async proxy) reads after the acquire
-        int target = pr.dep_target;
-        if (pr.dep_span != 0) {
-          const int lo = t.m_blk * pr.dep_span;
-          const int hi = lo + pr.dep_span < pr.dep_src_blocks ? lo + pr.dep_span : pr.dep_src_blocks;
-          target = (hi - lo) * pr.dep_per;
-        }
-        wait_counter_at_least(pr.dep_counter + (t.m_blk >> pr.dep_shift), target);
-        fence_proxy_async_all();
-      }
-      if (pr.kind == 1) {
-        // KV-attention tile: y_k . W_ik(head pair)^T, then y_v . W_iv(head pair)^T, through the same ring
-        const AttnParams& at = pr.attn;
-        if (at.k_counter != nullptr) {
-          // y_k / y_v were stored window-major by raster-ordered GEMMs of this launch: wait for every raster row block of the
-          // crops this tile touches, and for the q' row block of its windows
-          const long long r_lo = static_cast<long long>(t.m_blk) * Cfg::kTileM;
-          const long long r_hi = r_lo + Cfg::kTileM < pr.M ? r_lo + Cfg::kTileM : pr.M;
-          const int n_blocks = (pr.M + Cfg::kTileM - 1) / Cfg::kTileM;
-          int b_lo = static_cast<int>((r_lo / 576) * 576 / Cfg::kTileM);
-          int b_hi = static_cast<int>((((r_hi - 1) / 576 + 1) * 576 + Cfg::kTileM - 1) / Cfg::kTileM);
-          if (b_hi > n_blocks) b_hi = n_blocks;
-          for (int b = b_lo; b < b_hi; ++b) {
-            wait_counter_at_least(at.k_counter + b, at.kv_target);
-            wait_counter_at_least(at.v_counter + b, at.kv_target);
-          }
-          if (at.q_counter != nullptr) wait_counter_at_least(at.q_counter + ((r_lo / (at.s * at.s)) >> 8), at.q_target);
-          fence_proxy_async_all();
-        }
-        for (int op = 0; op < 2; ++op) {            // phase K, then phase V: two ordinary 256-wide k-loops (brow0: my half of the head pair's weight rows)
-          const CUtensorMap* ta = op == 0 ? &pr.tmap_a : &pr.tmap_a2;
-          const CUtensorMap* tb = op == 0 ? &pr.tmap_b : &pr.tmap_b2;
-          for (int kb = 0; kb < pr.num_k_blocks; ++kb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1u);
-            if (elect_one()) {
-              uint8_t* sa = smem + stage * Cfg::kStageBytes;
-              if (is_leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-              else mbar_arrive_cluster(&full_bar[stage], 0);
-              tma_load_2d_pair(sa, ta, &full_bar[stage], kb * kBlockK, row0);
-              tma_load_2d_pair(sa + Cfg::kABytes, tb, &full_bar[stage], kb * kBlockK, brow0);
-            }
-            __syncwarp();
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
-          }
-        }
-        continue;
-      }
-      int seg0 = 0, srow0 = 0, seg1 = 0, srow1 = 0;
-      if (pr.a_seg_rows != 0) {
-        seg0 = row0 / pr.a_seg_rows;
-        srow0 = row0 - seg0 * pr.a_seg_rows;
-        seg1 = (row0 + 64) / pr.a_seg_rows;
-        srow1 = row0 + 64 - seg1 * pr.a_seg_rows;
-      }
-      for (int kb = t.kb0; kb < t.kb1; ++kb) {
-        {
-          TP_PROF_T0();
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          TP_PROF_ADD(w_empty);
-        }
-        if (elect_one()) {
-          uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          uint8_t* sb = sa + Cfg::kABytes;
-          if (is_leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-          else mbar_arrive_cluster(&full_bar[stage], 0);
-          if (pr.ab_mn_major == 1) {
-            // boxes of [64 K-rows x 64 MN-elements]: coordinates (mn, k); two MN atoms per operand per CTA
-            tma_load_2d_pair(sa, &pr.tmap_a, &full_bar[stage], row0, kb * kBlockK);
-            tma_load_2d_pair(sa + Cfg::kABytes / 2, &pr.tmap_a, &full_bar[stage], row0 + 64, kb * kBlockK);
-          } else {
-            const int part = pr.a_parts > 1 ? kb / pr.a_kblocks_per_part : 0;
-            const CUtensorMap* ta = part == 0 ? &pr.tmap_a : &pr.tmap_a_more[part - 1];
-            const int ka = (kb - part * pr.a_kblocks_per_part) * kBlockK;      // K coordinate inside this part
-            if (pr.a_seg_rows == 0) {
-              tma_load_2d_pair(sa, ta, &full_bar[stage], ka, row0);
-            } else {
-              tma_load_3d_pair(sa, ta, &full_bar[stage], ka, srow0, seg0);
-              tma_load_3d_pair(sa + Cfg::kABytes / 2, ta, &full_bar[stage], ka, srow1, seg1);
-            }
-          }
-          if (pr.ab_mn_major == 0) {
-            tma_load_2d_pair(sb, &pr.tmap_b, &full_bar[stage], kb * kBlockK, brow0);
-          } else {                                       // 1 (TN) and 2 (NN): B is a row-major [K, N] matrix
-            tma_load_2d_pair(sb, &pr.tmap_b, &full_bar[stage], brow0, kb * kBlockK);
-            tma_load_2d_pair(sb + Cfg::kBBytes / 2, &pr.tmap_b, &full_bar[stage], brow0 + 64, kb * kBlockK);
-          }
-        }
-        __syncwarp();
-        if (++stage == kStages) { stage = 0; phase ^= 1u; }
-      }
-    }
-#ifdef TP_GEMM_PROFILE
-    if (grp.p[0].ep.prof != nullptr && lane == 0) {
-      grp.p[0].ep.prof[blockIdx.x * 16 + 0] = w_empty;
-      grp.p[0].ep.prof[blockIdx.x * 16 + 1] = clock64() - t_begin;
-    }
-#endif
-  } else if (warp_idx == kMmaWarp) {
-    // ======================================= MMA issuer (leader CTA only) ========================
-    if (is_leader) {
-      int stage = 0, cursor = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      [[maybe_unused]] long long w_full = 0, w_tmem = 0;
-      [[maybe_unused]] const long long t_begin = clock64();
-      for (int tile = pair_idx; tile < num_tiles; tile += num_pairs) {
-        const TileRef mt = decode_tile(grp, tile, cursor);
-        const GemmProblem& mpr = *mt.pr;
-        const int mn_major = mpr.ab_mn_major;
-        const uint32_t idesc = mn_major == 1 ? make_idesc_bf16_f32(Cfg::kTileM, kTileN, 1, 1)
-                             : mn_major == 2 ? make_idesc_bf16_f32(Cfg::kTileM, kTileN, 0, 1) : make_idesc_bf16_f32(Cfg::kTileM, kTileN);
-        {
-          TP_PROF_T0();
-          mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u);   // both epilogues have drained this accumulator buffer
-          TP_PROF_ADD(w_tmem);
-        }
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + static_cast<uint32_t>(acc * kTileN);
-        if (mpr.kind == 1) {
-          // phase K into this accumulator buffer, phase V into the other one: two ordinary 256 x 256 k-loops, each handed to the
-          // epilogue on its own (the wait on tmem_empty above covered phase K's buffer)
-          constexpr uint32_t idesc_kv = make_idesc_bf16_f32(Cfg::kTileM, kTileN);
-          for (int op = 0; op < 2; ++op) {
-            if (op == 1) {
-              mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u);
-              tcgen05_fence_after();
-            }
-            const uint32_t tmem_kv = tmem_base + static_cast<uint32_t>(acc * kTileN);
-            for (int kb = 0; kb < mpr.num_k_blocks; ++kb) {
-              mbar_wait(&full_bar[stage], phase);
-              tcgen05_fence_after();
-              if (elect_one()) {
-                const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-                const uint64_t desc_a = make_smem_desc_kmajor_sw128(sa);
-                const uint64_t desc_b = make_smem_desc_kmajor_sw128(sa + Cfg::kABytes);
-#pragma unroll
-                for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                  umma_bf16_pair(tmem_kv, desc_a + static_cast<uint64_t>(k * 2), desc_b + static_cast<uint64_t>(k * 2), idesc_kv,
-                                 static_cast<uint32_t>((kb | k) != 0));
-                }
-                umma_commit_pair(&empty_bar[stage], 0x3);
-                if (kb == mpr.num_k_blocks - 1) umma_commit_pair(&tmem_full_bar[acc], 0x3);
-              }
-              __syncwarp();
-              if (++stage == kStages) { stage = 0; phase ^= 1u; }
-            }
-            if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-          }
-          continue;
-        }
-        for (int kb = mt.kb0; kb < mt.kb1; ++kb) {
-          {
-            TP_PROF_T0();
-            mbar_wait(&full_bar[stage], phase);              // both CTAs' boxes have landed
-            TP_PROF_ADD(w_full);
-          }
-          tcgen05_fence_after();
-          if (elect_one()) {
-            const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-            if (mn_major == 2) {
-              // NN (dgrad: B = the weight as stored, row-major [K, N]): K-major A tile, MN-major B tile
-              const uint64_t desc_a = make_smem_desc_kmajor_sw128(sa);
-              const uint64_t desc_b = make_smem_desc_mnmajor_sw128(sa + Cfg::kABytes, Cfg::kBBytes / 2);
-#pragma unroll
-              for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                umma_bf16_pair(tmem_d, desc_a + static_cast<uint64_t>(k * 2), desc_b + static_cast<uint64_t>(k * (2048 >> 4)), idesc,
-                               static_cast<uint32_t>(((kb - mt.kb0) | k) != 0));
-              }
-            } else if (!mn_major) {
-              const uint64_t desc_a = make_smem_desc_kmajor_sw128(sa);
-              const uint64_t desc_b = make_smem_desc_kmajor_sw128(sa + Cfg::kABytes);
-#pragma unroll
-              for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                umma_bf16_pair(tmem_d, desc_a + static_cast<uint64_t>(k * 2), desc_b + static_cast<uint64_t>(k * 2), idesc,
-                               static_cast<uint32_t>(((kb - mt.kb0) | k) != 0));
-              }
-            } else {
-              // MN-major tiles: two 64-wide MN atoms 8 KiB apart per operand; one UMMA (K = 16) consumes two 8-row K groups = 2 KiB
-              const uint64_t desc_a = make_smem_desc_mnmajor_sw128(sa, Cfg::kABytes / 2);
-              const uint64_t desc_b = make_smem_desc_mnmajor_sw128(sa + Cfg::kABytes, Cfg::kBBytes / 2);
-#pragma unroll
-              for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-                umma_bf16_pair(tmem_d, desc_a + static_cast<uint64_t>(k * (2048 >> 4)), desc_b + static_cast<uint64_t>(k * (2048 >> 4)), idesc,
-                               static_cast<uint32_t>(((kb - mt.kb0) | k) != 0));
-              }
-            }
-            umma_commit_pair(&empty_bar[stage], 0x3);        // frees the slot in BOTH CTAs
-            if (kb == mt.kb1 - 1) umma_commit_pair(&tmem_full_bar[acc], 0x3);   // accumulator complete -> both epilogues
-          }
-          __syncwarp();
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-      }
-#ifdef TP_GEMM_PROFILE
-      if (grp.p[0].ep.prof != nullptr && lane == 0) {
-        grp.p[0].ep.prof[blockIdx.x * 16 + 2] = w_full;
-        grp.p[0].ep.prof[blockIdx.x * 16 + 3] = w_tmem;
-        grp.p[0].ep.prof[blockIdx.x * 16 + 4] = clock64() - t_begin;
-      }
-#endif
-    }
-  } else if (warp_idx >= kEpiWarp0 && warp_idx < kEpiWarp0 + kNumEpiWarps) {
-    // ======================================= epilogue (both CTAs, own 128 rows) ==================
+  if (warp_idx < kNumEpiWarps) {
+    setmaxnreg_inc<kMmaRegs>();
+    // ======================================= MMA + epilogue (own 128 rows, warpgroup = column half) ==
     const int e = warp_idx - kEpiWarp0;
     const int quarter = warp_idx & 3;
     const int half = e >> 2;
     const int epi_tid = e * 32 + static_cast<int>(lane);
-    int acc = 0, cursor = 0;
-    uint32_t acc_phase = 0;
+    const uint32_t scratch = smem_u32(s_scratch + e * kScratchBytesPerWarp);
+    const int b_off = half * kN * kBlockK * 2;                  // this warpgroup's columns of the stage's B tile
+    int cursor = 0, stage = 0;
+    uint32_t phase = 0;
     uint32_t slab_seq = 0;
+    float acc[2][kN / 2];
     [[maybe_unused]] long long w_acc = 0, t_work = 0;
     [[maybe_unused]] long long pc[3] = {0, 0, 0};
     if (grp.front.x0 != nullptr) {
@@ -1144,37 +938,22 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       const TileRef t = decode_tile(grp, tile, cursor);
       const GemmProblem& pr = *t.pr;
       float* s_col = s_col_base;
-      uint64_t* release_bar = &tmem_empty_bar[acc];
       const int row_tile0 = t.m_blk * Cfg::kTileM + static_cast<int>(cta_rank) * kBlockM;
-      const int row = row_tile0 + quarter * 32 + static_cast<int>(lane);
+      const int row = row_tile0 + epi_row(quarter, lane);
       if (pr.kind == 1) {
         const AttnParams& at = pr.attn;
         const int head = t.n_blk * 2 + half;                 // column half == head of the tile's pair
-        auto release_acc = [&](uint64_t* bar) {
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if (is_leader) mbar_arrive(bar);
-            else mbar_arrive_cluster(bar, 0);
-          }
-        };
         GemmEpilogue vec;                                    // only col_a / col_b are read by the staging helper
         vec.col_a = at.wsum_k;
         vec.col_b = at.cst_k;
         stage_col_vectors<kTileN>(vec, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
-        mbar_wait(&tmem_full_bar[acc], acc_phase);
-        tcgen05_fence_after();
-        const float p = attn_scores(at, pr.M, tmem_base + static_cast<uint32_t>(acc * kTileN), row, head, quarter, half, s_col,
-                                    [&]() { release_acc(release_bar); });
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-        float* s_col_v = s_col_base;
+        mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
+        const float p = attn_scores(at, pr.M, acc, scratch, row, head, half, s_col);
         vec.col_a = at.wsum_v;
         vec.col_b = at.cst_v;
-        stage_col_vectors<kTileN>(vec, pr.N, t.n_blk * kTileN, s_col_v, epi_tid, true);
-        mbar_wait(&tmem_full_bar[acc], acc_phase);
-        tcgen05_fence_after();
-        uint64_t* release_v = &tmem_empty_bar[acc];
-        attn_pv(at, pr.M, tmem_base + static_cast<uint32_t>(acc * kTileN), row, head, quarter, half, p, s_col_v, [&]() { release_acc(release_v); });
+        stage_col_vectors<kTileN>(vec, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
+        mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
+        attn_pv(at, pr.M, acc, scratch, row, head, half, p, s_col);
         if (at.done_counter != nullptr) {
           named_bar_sync(kEpiBarrierId, kEpiThreads);       // every epilogue thread's ctx stores are issued ...
           if (epi_tid == 0) {
@@ -1182,44 +961,153 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
             red_release_gpu_add(at.done_counter + ((static_cast<long long>(t.m_blk) * Cfg::kTileM / (at.s * at.s)) >> 8), 1);
           }
         }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
         continue;
       }
       stage_col_vectors<kTileN>(pr.ep, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
       {
         TP_PROF_T0();
-        mbar_wait(&tmem_full_bar[acc], acc_phase);
+        const int n_kb = t.kb1 - t.kb0;
+        if (pr.ab_mn_major == 1)
+          mma_tile<kN, 1, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
+        else if (pr.ab_mn_major == 2)
+          mma_tile<kN, 0, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
+        else
+          mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
         TP_PROF_ADD(w_acc);
       }
       TP_PROF_T0();
-      tcgen05_fence_after();
       const OutStage out{pr.use_tma_store ? s_out + half * Cfg::kOutBufs * kOutSlabBytes : nullptr, slab_full_bar + half * Cfg::kOutBufs,
                          slab_empty_bar + half * Cfg::kOutBufs, Cfg::kOutBufs, slab_seq, pr.c_noswz == 0};
       if (pr.use_tma_store) slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);     // slabs per tile and column half
-      epilogue_tile<kTileN>(pr.ep, pr.M, pr.N, tmem_base + static_cast<uint32_t>(acc * kTileN), row, t.n_blk * kTileN, quarter, half, s_col,
-                            out, [&]() {
-                              tcgen05_fence_before();
-                              __syncwarp();
-                              if (lane == 0) {
-                                if (is_leader) mbar_arrive(release_bar);
-                                else mbar_arrive_cluster(release_bar, 0);
-                              }
-                            }, pc, static_cast<long long>(t.split) * pr.c_split_stride);
+      epilogue_tile<kTileN>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, quarter, half, s_col, out, pc,
+                            static_cast<long long>(t.split) * pr.c_split_stride);
       TP_PROF_ADD(t_work);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
     }
 #ifdef TP_GEMM_PROFILE
     if (grp.p[0].ep.prof != nullptr && e == 0 && lane == 0) {
       grp.p[0].ep.prof[blockIdx.x * 16 + 5] = w_acc;
       grp.p[0].ep.prof[blockIdx.x * 16 + 6] = t_work;
-      grp.p[0].ep.prof[blockIdx.x * 16 + 8] = pc[0];          // epilogue warp 0: cycles in tcgen05.wait::ld
+      grp.p[0].ep.prof[blockIdx.x * 16 + 8] = pc[0];          // epilogue warp 0: cycles in the accumulator transpose
       grp.p[0].ep.prof[blockIdx.x * 16 + 9] = pc[1];         // ... in fence.proxy.async
       grp.p[0].ep.prof[blockIdx.x * 16 + 10] = pc[2];          // ... in wait_group.read + named barrier
     }
 #endif
-  }
-
-  if (warp_idx == kStoreWarp0 || warp_idx == kStoreWarp0 + 1) {
+  } else {
+    setmaxnreg_dec<kAuxRegs>();
+  if (warp_idx == kTmaWarp) {
+    // ======================================= TMA producer (both CTAs) ============================
+    // Whole warp runs the loop (uniform control flow); one elected lane issues the arrive + TMA instructions.
+    int stage = 0, cursor = 0;
+    uint32_t phase = 0;
+    [[maybe_unused]] long long w_empty = 0;
+    [[maybe_unused]] const long long t_begin = clock64();
+    for (int tile = pair_idx; tile < num_tiles; tile += num_pairs) {
+      const TileRef t = decode_tile(grp, tile, cursor);
+      const GemmProblem& pr = *t.pr;
+      const int row0 = t.m_blk * Cfg::kTileM + static_cast<int>(cta_rank) * kBlockM;          // my 128 rows of A
+      const int brow0 = t.n_blk * kTileN;                                                     // the whole B tile
+      // segmented A (3-D map, 64-row boxes): global row g -> (segment g / seg_rows, row g % seg_rows); hoisted per tile
+      if (pr.dep_counter != nullptr) {
+        // A's row block is written by an earlier problem of this launch: wait until all its tiles have been published (acquire),
+        // then order the TMA (async proxy) reads after the acquire
+        int target = pr.dep_target;
+        if (pr.dep_span != 0) {
+          const int lo = t.m_blk * pr.dep_span;
+          const int hi = lo + pr.dep_span < pr.dep_src_blocks ? lo + pr.dep_span : pr.dep_src_blocks;
+          target = (hi - lo) * pr.dep_per;
+        }
+        wait_counter_at_least(pr.dep_counter + (t.m_blk >> pr.dep_shift), target);
+        fence_proxy_async_all();
+      }
+      if (pr.kind == 1) {
+        // KV-attention tile: y_k . W_ik(head pair)^T, then y_v . W_iv(head pair)^T, through the same ring
+        const AttnParams& at = pr.attn;
+        if (at.k_counter != nullptr) {
+          // y_k / y_v were stored window-major by raster-ordered GEMMs of this launch: wait for every raster row block of the
+          // crops this tile touches, and for the q' row block of its windows
+          const long long r_lo = static_cast<long long>(t.m_blk) * Cfg::kTileM;
+          const long long r_hi = r_lo + Cfg::kTileM < pr.M ? r_lo + Cfg::kTileM : pr.M;
+          const int n_blocks = (pr.M + Cfg::kTileM - 1) / Cfg::kTileM;
+          int b_lo = static_cast<int>((r_lo / 576) * 576 / Cfg::kTileM);
+          int b_hi = static_cast<int>((((r_hi - 1) / 576 + 1) * 576 + Cfg::kTileM - 1) / Cfg::kTileM);
+          if (b_hi > n_blocks) b_hi = n_blocks;
+          for (int b = b_lo; b < b_hi; ++b) {
+            wait_counter_at_least(at.k_counter + b, at.kv_target);
+            wait_counter_at_least(at.v_counter + b, at.kv_target);
+          }
+          if (at.q_counter != nullptr) wait_counter_at_least(at.q_counter + ((r_lo / (at.s * at.s)) >> 8), at.q_target);
+          fence_proxy_async_all();
+        }
+        for (int op = 0; op < 2; ++op) {            // phase K, then phase V: two ordinary 256-wide k-loops (brow0: the head pair's weight rows)
+          const CUtensorMap* ta = op == 0 ? &pr.tmap_a : &pr.tmap_a2;
+          const CUtensorMap* tb = op == 0 ? &pr.tmap_b : &pr.tmap_b2;
+          for (int kb = 0; kb < pr.num_k_blocks; ++kb) {
+            mbar_wait(&empty_bar[stage], phase ^ 1u);
+            if (elect_one()) {
+              uint8_t* sa = smem + stage * Cfg::kStageBytes;
+              mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+              tma_load_2d(sa, ta, &full_bar[stage], kb * kBlockK, row0);
+              tma_load_2d(sa + Cfg::kABytes, tb, &full_bar[stage], kb * kBlockK, brow0);
+              tma_load_2d(sa + Cfg::kABytes + Cfg::kBBytes / 2, tb, &full_bar[stage], kb * kBlockK, brow0 + kTileN / 2);
+            }
+            __syncwarp();
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
+        }
+        continue;
+      }
+      int seg0 = 0, srow0 = 0, seg1 = 0, srow1 = 0;
+      if (pr.a_seg_rows != 0) {
+        seg0 = row0 / pr.a_seg_rows;
+        srow0 = row0 - seg0 * pr.a_seg_rows;
+        seg1 = (row0 + 64) / pr.a_seg_rows;
+        srow1 = row0 + 64 - seg1 * pr.a_seg_rows;
+      }
+      for (int kb = t.kb0; kb < t.kb1; ++kb) {
+        {
+          TP_PROF_T0();
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          TP_PROF_ADD(w_empty);
+        }
+        if (elect_one()) {
+          uint8_t* sa = smem + stage * Cfg::kStageBytes;
+          uint8_t* sb = sa + Cfg::kABytes;
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          if (pr.ab_mn_major == 1) {
+            // boxes of [64 K-rows x 64 MN-elements]: coordinates (mn, k); two MN atoms of A, four of B per CTA
+            tma_load_2d(sa, &pr.tmap_a, &full_bar[stage], row0, kb * kBlockK);
+            tma_load_2d(sa + Cfg::kABytes / 2, &pr.tmap_a, &full_bar[stage], row0 + 64, kb * kBlockK);
+          } else {
+            const int part = pr.a_parts > 1 ? kb / pr.a_kblocks_per_part : 0;
+            const CUtensorMap* ta = part == 0 ? &pr.tmap_a : &pr.tmap_a_more[part - 1];
+            const int ka = (kb - part * pr.a_kblocks_per_part) * kBlockK;      // K coordinate inside this part
+            if (pr.a_seg_rows == 0) {
+              tma_load_2d(sa, ta, &full_bar[stage], ka, row0);
+            } else {
+              tma_load_3d(sa, ta, &full_bar[stage], ka, srow0, seg0);
+              tma_load_3d(sa + Cfg::kABytes / 2, ta, &full_bar[stage], ka, srow1, seg1);
+            }
+          }
+          if (pr.ab_mn_major == 0) {
+            tma_load_2d(sb, &pr.tmap_b, &full_bar[stage], kb * kBlockK, brow0);
+            tma_load_2d(sb + Cfg::kBBytes / 2, &pr.tmap_b, &full_bar[stage], kb * kBlockK, brow0 + kTileN / 2);
+          } else {                                       // 1 (TN) and 2 (NN): B is a row-major [K, N] matrix
+#pragma unroll
+            for (int a4 = 0; a4 < 4; ++a4)
+              tma_load_2d(sb + a4 * (Cfg::kBBytes / 4), &pr.tmap_b, &full_bar[stage], brow0 + a4 * 64, kb * kBlockK);
+          }
+        }
+        __syncwarp();
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
+      }
+    }
+#ifdef TP_GEMM_PROFILE
+    if (grp.p[0].ep.prof != nullptr && lane == 0) {
+      grp.p[0].ep.prof[blockIdx.x * 16 + 0] = w_empty;
+      grp.p[0].ep.prof[blockIdx.x * 16 + 1] = clock64() - t_begin;
+    }
+#endif
+  } else if (warp_idx == kStoreWarp0 || warp_idx == kStoreWarp0 + 1) {
     // ======================================= store warps (both CTAs, one per column half) =========
     // Walks the same tile sequence as the epilogue warps of its half.  Per slab: wait until the 4 epilogue warps have written
     // it (mbarrier), issue the TMA store(s) — plain 2-D box, clipped 3-D boxes for segmented rows, one per peer GPU for the
@@ -1259,7 +1147,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
               if (job == static_cast<int>(lane) + 32 * k) { jmap[k] = mp; jlo[k] = lo; jc1[k] = c1; jc2[k] = c2; jc3[k] = c3; jc4[k] = c4; }
             ++job;
           };
-          // TMA stores must lie entirely inside the tensor (a box that sticks out of a segment faults: measured), so every piece of
+          // TMA stores must lie entirely inside the tensor (a box that sticks out of a segment is not relied on), so every piece of
           // a slab goes out through boxes of EXACTLY its size: a few maps per destination with box heights unit << level.
           int kind = 2;                                    // dimensionality of this problem's stores: 2, 3 or 5
           if (pr.c_wm_s != 0) {
@@ -1341,12 +1229,6 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
     if (peers.count > 0) __threadfence_system();   // ... and are ordered before the cross-GPU barrier that follows the kernel
     __syncwarp();
   }
-
-  tcgen05_fence_before();
-  cluster_sync_all();                      // the peer may read my smem / signal my barriers until here
-  if (warp_idx == kAllocWarp) {
-    tcgen05_fence_after();
-    tmem_dealloc_pair<Cfg::kTmemCols>(tmem_base);
   }
 }
 

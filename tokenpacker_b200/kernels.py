@@ -8,7 +8,7 @@ from ._lib import lib, check
 
 def gemm_bf16(a: torch.Tensor, b: torch.Tensor, bias: torch.Tensor | None = None, gelu: bool = False, alpha: float = 1.0,
               out: torch.Tensor | None = None) -> torch.Tensor:
-    """C[M,N] = alpha * act(A[M,K] @ B[N,K]^T + bias): the tcgen05 GEMM every nn.Linear of the path runs on.
+    """C[M,N] = alpha * act(A[M,K] @ B[N,K]^T + bias): the wgmma GEMM every nn.Linear of the path runs on.
     a, b: bf16 CUDA, unit inner stride; bias: fp32 [N] or None."""
     if not (a.is_cuda and b.is_cuda) or a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16:
         raise TypeError("gemm_bf16 needs bf16 CUDA tensors (no CPU path)")

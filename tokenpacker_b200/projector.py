@@ -133,7 +133,7 @@ class TokenPackerB200(nn.Module):
         if raw_grid % scale_factor != 0:
             raise ValueError("scale_factor must be divisible by grid size")      # builder.py:51-52, same message
         if (raw_grid, embed_dim, num_heads, kv_dim) != (24, 1024, 8, 1024):
-            raise NotImplementedError("the sm_100a kernels are specialised for CLIP-ViT-L/14-336: raw_grid=24, "
+            raise NotImplementedError("the sm_90a kernels are specialised for CLIP-ViT-L/14-336: raw_grid=24, "
                                       "embed_dim=kv_dim=1024, num_heads=8 (the only configuration the reference builds)")
         if hidden_size % 32 != 0:
             raise NotImplementedError("hidden_size must be a multiple of 32")
@@ -242,7 +242,7 @@ class TokenPackerB200(nn.Module):
                 or x0.shape[0] != xm.shape[0]:
             raise ValueError(f"expected feat [N,576,1024] and feat_multi [N,576,4096], got {tuple(x0.shape)} {tuple(xm.shape)}")
         if not (x0.is_cuda and xm.is_cuda):
-            raise RuntimeError("tokenpacker_b200 has no CPU path: inputs must be CUDA tensors on a B200")
+            raise RuntimeError("tokenpacker_b200 has no CPU path: inputs must be CUDA tensors on an H100")
         if not self._warned_dtype and (x0.dtype != torch.bfloat16 or self._raw_params()[0].dtype != torch.bfloat16):
             self._warned_dtype = True
             warnings.warn("tokenpacker_b200 computes with bf16 storage and fp32 accumulation: fp16 / fp32 inputs and parameters are cast to "
@@ -361,7 +361,7 @@ class TokenPackerB200(nn.Module):
         n = x0.shape[0]
         device = torch.device(device if device is not None else next(self.parameters()).device)
         if device.type != "cuda":
-            raise RuntimeError("tokenpacker_b200 has no CPU path: move the module to a B200 first")
+            raise RuntimeError("tokenpacker_b200 has no CPU path: move the module to an H100 first")
         if out is None:
             out = torch.empty((n, self.num_queries, self.hidden_size), dtype=torch.bfloat16).pin_memory()
         with torch.cuda.device(device):
@@ -416,7 +416,7 @@ class TokenPackerB200(nn.Module):
         return (out if x0.dtype == torch.bfloat16 else out.to(x0.dtype)), plan.cu_seqlens
 
     def extra_repr(self):
-        return f"scale_factor={self.scale_factor}, num_queries={self.num_queries}, hidden_size={self.hidden_size}, backend=sm_100a"
+        return f"scale_factor={self.scale_factor}, num_queries={self.num_queries}, hidden_size={self.hidden_size}, backend=sm_90a"
 
 
 # the reference's class name, so `from ...builder import TokenPacker` style imports can be redirected unchanged
