@@ -37,7 +37,7 @@ typedef enum tp_status {
   TP_ERR_BAD_SCALE_FACTOR = 2, /* 24 % scale_factor != 0  (reference: ValueError, builder.py:51-52) */
   TP_ERR_WORKSPACE_TOO_SMALL = 3,
   TP_ERR_CUDA = 4,             /* a CUDA runtime / driver call failed; see tp_last_cuda_error() */
-  TP_ERR_UNSUPPORTED_DEVICE = 5, /* not a compute-capability 10.x device */
+  TP_ERR_UNSUPPORTED_DEVICE = 5, /* not a compute-capability 9.x device */
   TP_ERR_BAD_PATCH_NUM = 6     /* patch_num not in {9,16,25} (reference: NotImplementedError, patch_divide.py:79-80) */
 } tp_status;
 

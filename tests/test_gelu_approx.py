@@ -29,11 +29,12 @@ def _coefficients():
 
 
 def gelu_device(x):
-    """The instruction sequence of gelu_erf: t = |x|/sqrt2; Horner (6 fma); 4 squarings; one reciprocal; e = 1 - r;
-    0.5 * fma(|x|, e, x)."""
+    """The instruction sequence of gelu_erf: h = x/2; t = |h| sqrt2; Horner (6 fma); 4 squarings; one reciprocal; e = 1 - r;
+    fma(|h|, e, h)."""
     x = x.astype(f32)
-    ax = np.abs(x)
-    t = (ax * f32(0.70710678118654752440)).astype(f32)
+    h = (f32(0.5) * x).astype(f32)
+    ah = np.abs(h)
+    t = (ah * f32(1.41421356237309504880)).astype(f32)
     c = _coefficients()
     p = np.full_like(x, c[0])
     for coef in c[1:]:
@@ -43,7 +44,7 @@ def gelu_device(x):
             p = (p * p).astype(f32)                      # +inf for |x| > ~24 -> r = 0 -> erf = 1
         r = (f32(1.0) / p).astype(f32)                   # MUFU.RCP: within 1 ulp of this
     e = (f32(1.0) - r).astype(f32)
-    return (f32(0.5) * _fma(ax, e, x)).astype(f32)
+    return _fma(ah, e, h)
 
 
 def test_coefficients_are_abramowitz_stegun_7_1_28():
@@ -77,3 +78,22 @@ def test_limits():
     x = np.array([40.0, -40.0, 0.0], dtype=f32)
     y = gelu_device(x)
     assert y[0] == f32(40.0) and y[1] == 0.0 and y[2] == 0.0
+
+
+def test_no_overflow_at_the_top_of_the_range():
+    """GELU(x) = x for large x: 0.5 * (x + |x| e) evaluated as written reaches 2x = +inf for x >= 2^127."""
+    big = np.finfo(f32).max
+    x = np.array([2.0 ** 127, big, -(2.0 ** 127), -big], dtype=f32)
+    with np.errstate(over="ignore"):
+        y = gelu_device(x)
+    assert y[0] == x[0] and y[1] == x[1] and y[2] == 0.0 and y[3] == 0.0
+
+
+def test_halving_first_keeps_the_bits_of_the_unhalved_form():
+    """h = x/2 is exact for |x| >= 2^-125, and then fma(|h|, e, h) = 0.5 * fma(|x|, e, x) and |h| sqrt2 = |x| / sqrt2 bit for bit."""
+    rng = np.random.default_rng(0)
+    x = np.concatenate([rng.standard_normal(200000) * 4, np.linspace(-30, 30, 60001)]).astype(f32)
+    h = (f32(0.5) * x).astype(f32)
+    assert np.array_equal((np.abs(h) * f32(1.41421356237309504880)).astype(f32), (np.abs(x) * f32(0.70710678118654752440)).astype(f32))
+    e = rng.random(x.shape).astype(f32)
+    assert np.array_equal(_fma(np.abs(h), e, h), (f32(0.5) * _fma(np.abs(x), e, x)).astype(f32))
