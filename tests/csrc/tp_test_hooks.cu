@@ -1,5 +1,5 @@
-// Test-only entry points into the backward's internal kernels (libtokenpacker_b200_testhooks.so, loaded by
-// tests/test_train_kernels_gpu.py; never by the package).  The library is the product translation unit plus the tpt_* functions
+// Test-only entry points into the backward's internal kernels and the forward's buffer layouts (libtokenpacker_b200_testhooks.so,
+// loaded by tests/test_train_kernels_gpu.py and tests/test_forward_stages_gpu.py; never by the package).  The library is the product translation unit plus the tpt_* functions
 // below, which call the same launch functions tp_backward calls (tp_train.inl), so every kernel runs with the launch configuration
 // of a training step.  Conventions as in include/tokenpacker_b200.h: device pointers, caller-owned buffers, work enqueued on
 // ``stream``, a tp_status returned.
@@ -88,6 +88,37 @@ TP_API int tpt_colsum(const void* in, int64_t ld, int64_t rows, int cols, float 
                       void* stream) {
   if (in == nullptr || out == nullptr || partial == nullptr || rows <= 0 || cols <= 0 || ld % 8 != 0) return TP_ERR_INVALID_ARGUMENT;
   return bias_grad(in, ld, rows, cols, scale, out, partial, partial_floats, static_cast<cudaStream_t>(stream));
+}
+
+// Workspace layout of tp_forward for (n_crops, s, hidden), so that a test reads each stage's output where the forward put it:
+// out[2 i], out[2 i + 1] = byte offset and byte size of region i in WorkLayout order (h_kv, y_k, y_v, k_p, v_p, stats, q, y_q, q_p,
+// ctx, h_m, flags); out[24] = total.  The sizes are the regions' shapes (WorkLayout's comments); the gaps up to the next offset are
+// alignment padding that nothing writes.
+TP_API int tpt_work_layout(int64_t n_crops, int s, int hidden, int64_t* out) {
+  if (out == nullptr || n_crops <= 0 || s <= 0 || kGrid % s != 0 || !valid_hidden(hidden)) return TP_ERR_INVALID_ARGUMENT;
+  const WorkLayout L = work_layout(n_crops, s, hidden);
+  const long long R = n_crops * kTokens, Q = n_crops * (kGrid / s) * (kGrid / s);
+  const size_t off[12] = {L.h_kv, L.y_k, L.y_v, L.k_p, L.v_p, L.stats, L.q, L.y_q, L.q_p, L.ctx, L.h_m, L.flags};
+  const long long bytes[12] = {R * 2 * kC * 2, R * kC * 2, R * kC * 2, R * kC * 2, R * kC * 2, (2 * R + Q) * kStatSlots * 2 * 4,
+                               Q * kC * 2, Q * kC * 2, Q * kC * 2, Q * kC * 2, Q * hidden * 2, L.n_flags * 4};
+  for (int i = 0; i < 12; ++i) {
+    out[2 * i] = static_cast<int64_t>(off[i]);
+    out[2 * i + 1] = bytes[i];
+  }
+  out[24] = static_cast<int64_t>(L.total);
+  return TP_OK;
+}
+
+// Packed-weight layout of tp_pack_weights for hidden: every PackedLayout byte offset in declaration order (w_kv0, b_kv0, w_k2, b_k2,
+// w_v2, b_v2, w_ik, wsum_k, c_k, w_iv, wsum_v, c_v, w_q, w_iq, wsum_q, c_q, w_ot, w_om, b_om, w_m2, b_m2, w_o, b_o, w_m0, b_m0), then
+// the total: 26 values.
+TP_API int tpt_packed_layout(int hidden, int64_t* out) {
+  if (out == nullptr || !valid_hidden(hidden)) return TP_ERR_INVALID_ARGUMENT;
+  const PackedLayout L = packed_layout(hidden);
+  const size_t f[26] = {L.w_kv0, L.b_kv0, L.w_k2, L.b_k2, L.w_v2, L.b_v2, L.w_ik, L.wsum_k, L.c_k, L.w_iv, L.wsum_v, L.c_v, L.w_q,
+                        L.w_iq, L.wsum_q, L.c_q, L.w_ot, L.w_om, L.b_om, L.w_m2, L.b_m2, L.w_o, L.b_o, L.w_m0, L.b_m0, L.total};
+  for (int i = 0; i < 26; ++i) out[i] = static_cast<int64_t>(f[i]);
+  return TP_OK;
 }
 
 // out[c, r] = in[r, c]

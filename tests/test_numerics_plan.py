@@ -67,6 +67,59 @@ def device_plan_forward(p, x0, xm, s):
     return out.reshape(n, g * g, -1)
 
 
+def _stencil_f32(a, b, c, d):
+    """point_query_kernel's even-s sequence in float32 (numpy rounds every operation, no FMA): (0.25a + 0.25b) + (0.25c + 0.25d)"""
+    q = f32(0.25)
+    return (q * a + q * b) + (q * c + q * d)
+
+
+def _bf16_bits(rng, shape):
+    """random finite bf16 values over every binade, both signs, subnormals and zeros included"""
+    bits = rng.integers(0, 1 << 16, size=shape, dtype=np.uint32)
+    bits = np.where((bits & 0x7F80) == 0x7F80, bits & 0x807F, bits)        # inf / nan -> a subnormal of the same sign
+    return (bits << 16).view(np.float32)
+
+
+@pytest.mark.parametrize("s", [2, 4])
+def test_point_query_stencil_matches_interpolate_bits(s):
+    """The even-s stencil against torch's bilinear F.interpolate (the reference, builder.py:117-118): bit for bit, before and after
+    the bf16 rounding, on windows of subnormal taps and windows whose taps lie in bf16's top binade (|x| >= 2^127) with equal and
+    mixed signs; within two fp32 roundings on random bf16 taps from every binade.  Adding the taps before scaling them,
+    0.25 ((a + b) + (c + d)), overflows to inf on the top-binade windows and gives the same bits everywhere else: checked too, so
+    the inputs really reach the range the sequence is for."""
+    import torch
+    import torch.nn.functional as F
+    g, c = 24 // s, 64
+    rng = np.random.default_rng(7 + s)
+    img = _bf16_bits(rng, (c, 24, 24))
+    lo = s // 2 - 1                                              # first centre tap of a window
+    top = (rng.integers(0x7F00, 0x7F80, size=(c, 4), dtype=np.uint32) << 16).view(np.float32)     # [2^127, max bf16]
+    signs = np.array([[1, 1, 1, 1], [-1, -1, -1, -1], [1, -1, 1, -1], [1, 1, -1, 1]], dtype=np.float32)
+    sub = _bf16_bits(rng, (c, 4)).view(np.uint32) & np.uint32(0x807F0000)                          # subnormals and zeros
+    special = {(0, 0): top * signs[0], (0, 1): top * signs[1], (1, 0): top * signs[2], (1, 1): top * signs[3],
+               (2, 2): sub.view(np.float32), (g - 1, g - 1): np.full((c, 4), 2.0 ** 127, dtype=np.float32)}
+    for (hb, wb), taps in special.items():
+        r, cc = hb * s + lo, wb * s + lo
+        img[:, r, cc], img[:, r, cc + 1], img[:, r + 1, cc], img[:, r + 1, cc + 1] = taps.T
+    ref = F.interpolate(torch.from_numpy(img)[None], size=(g, g), mode="bilinear", align_corners=False)[0].numpy()
+    i = np.arange(g) * s + lo
+    a, b = img[:, i][:, :, i], img[:, i][:, :, i + 1]
+    cq, d = img[:, i + 1][:, :, i], img[:, i + 1][:, :, i + 1]
+    got = _stencil_f32(a, b, cq, d)
+    assert np.isfinite(got).all()
+    for hb, wb in special:
+        assert np.array_equal(got[:, hb, wb].view(np.uint32), ref[:, hb, wb].view(np.uint32)), (hb, wb)
+        assert np.array_equal(bf(got[:, hb, wb]).view(np.uint32), bf(ref[:, hb, wb]).view(np.uint32)), (hb, wb)
+    # elsewhere the taps span many binades, the fp32 sums round, and ATen adds in another order: both are within two roundings
+    mag = sum(np.abs(t.astype(np.float64)) for t in (a, b, cq, d)) * 0.25
+    assert (np.abs(got.astype(np.float64) - ref) <= 4 * 2.0 ** -24 * mag).all()
+    with np.errstate(over="ignore"):
+        old = f32(0.25) * ((a + b) + (cq + d))
+    assert np.isinf(old[:, 0, 0]).all() and np.isinf(old[:, g - 1, g - 1]).all()
+    fin = np.isfinite(old)                                       # elsewhere the two sequences give the same bits
+    assert np.array_equal(old[fin].view(np.uint32), got[fin].view(np.uint32))
+
+
 @pytest.mark.parametrize("s", [2, 3, 4, 6])
 def test_device_plan_meets_the_gpu_gates(s):
     hidden, n = 128, 2

@@ -918,11 +918,13 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
         if (!(fw.s & 1)) {
           const uint4 b = __ldg(reinterpret_cast<const uint4*>(base + 1024)), c = __ldg(reinterpret_cast<const uint4*>(base + 24 * 1024)),
                       d = __ldg(reinterpret_cast<const uint4*>(base + 25 * 1024));
-          // 0.25 * ((a + b) + (c + d)): the association of point_query_kernel (bit-identical; power-of-two scaling is exact)
+          // (0.25a + 0.25b) + (0.25c + 0.25d): the sequence of point_query_kernel, so both give the same bits; taps are scaled before
+          // the adds, so no partial sum overflows when taps lie in bf16's top binade
           auto mean4 = [](uint32_t a_, uint32_t b_, uint32_t c_, uint32_t d_) {
-            const float l = 0.25f * ((bf16_lo(a_) + bf16_lo(b_)) + (bf16_lo(c_) + bf16_lo(d_)));
-            const float h = 0.25f * ((bf16_hi(a_) + bf16_hi(b_)) + (bf16_hi(c_) + bf16_hi(d_)));
-            return pack_bf16x2(l, h);
+            auto m4 = [](float a, float b, float c, float d) {
+              return __fadd_rn(__fadd_rn(__fmul_rn(0.25f, a), __fmul_rn(0.25f, b)), __fadd_rn(__fmul_rn(0.25f, c), __fmul_rn(0.25f, d)));
+            };
+            return pack_bf16x2(m4(bf16_lo(a_), bf16_lo(b_), bf16_lo(c_), bf16_lo(d_)), m4(bf16_hi(a_), bf16_hi(b_), bf16_hi(c_), bf16_hi(d_)));
           };
           o = make_uint4(mean4(o.x, b.x, c.x, d.x), mean4(o.y, b.y, c.y, d.y), mean4(o.z, b.z, c.z, d.z), mean4(o.w, b.w, c.w, d.w));
         }

@@ -57,9 +57,13 @@ __global__ void point_query_kernel(const __nv_bfloat16* __restrict__ x0, long lo
     unpack8(tok(r0, c0 + 1), b);
     unpack8(tok(r0 + 1, c0), c);
     unpack8(tok(r0 + 1, c0 + 1), d);
-    // 0.5*(0.5a+0.5b) + 0.5*(0.5c+0.5d): scaling by powers of two is exact, so this association is bit-identical
+    // (0.25a + 0.25b) + (0.25c + 0.25d): each tap is scaled BEFORE the adds, so taps in bf16's top binade (|x| >= 2^127) cannot
+    // overflow a partial sum.  0.25 x is exact for every bf16 x (bf16's smallest subnormal is 2^-133, fp32's 2^-149), so the bits
+    // are those of the reference's 0.5 (0.5a + 0.5b) + 0.5 (0.5c + 0.5d), and — wherever the scaled taps and partial sums are
+    // normal numbers — those of the former 0.25 ((a + b) + (c + d)).  Explicit intrinsics: no FMA contraction.
 #pragma unroll
-    for (int i = 0; i < 8; ++i) o[i] = 0.25f * ((a[i] + b[i]) + (c[i] + d[i]));
+    for (int i = 0; i < 8; ++i)
+      o[i] = __fadd_rn(__fadd_rn(__fmul_rn(0.25f, a[i]), __fmul_rn(0.25f, b[i])), __fadd_rn(__fmul_rn(0.25f, c[i]), __fmul_rn(0.25f, d[i])));
     out = pack8(o);
   }
   *reinterpret_cast<uint4*>(q + query * kC + vec * 8) = out;
