@@ -1,7 +1,7 @@
 """ctypes binding of libtokenpacker_b200.so — the thin seam between the Python host code and the C-ABI CUDA library.
 
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
-Signatures mirror include/tokenpacker_b200.h one to one.
+Signatures mirror include/tokenpacker_b200.h and include/tokenpacker_b200_hd_u8.h one to one.
 """
 from __future__ import annotations
 
@@ -47,6 +47,12 @@ class TpHdImage(C.Structure):
     _fields_ = [("image", C.c_void_p), ("h", C.c_int32), ("w", C.c_int32), ("hb", C.c_int32), ("wb", C.c_int32),
                 ("h_r", C.c_int32), ("w_r", C.c_int32), ("h_t", C.c_int32), ("w_t", C.c_int32), ("crop0", C.c_int64),
                 ("sy", C.c_float), ("sx", C.c_float), ("ty", C.c_float), ("tx", C.c_float)]
+
+
+class TpHdU8Source(C.Structure):
+    """tp_hd_u8_source (include/tokenpacker_b200_hd_u8.h): where one decoded 8-bit image lies (element strides of channel, row
+    and column)."""
+    _fields_ = [("pixels", C.c_void_p), ("stride_c", C.c_int64), ("stride_y", C.c_int64), ("stride_x", C.c_int64)]
 
 
 # name -> (restype, argtypes); kept as data so tests can check the header and the binding agree
@@ -98,6 +104,11 @@ SIGNATURES = {
                                         C.c_void_p, C.c_void_p]),
 }
 
+# the same for include/tokenpacker_b200_hd_u8.h (decoded 8-bit images into the batched HD front end)
+HD_U8_SIGNATURES = {
+    "tp_hd_preprocess_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+}
+
 
 def _load():
     if not os.path.exists(LIB_PATH):
@@ -105,7 +116,7 @@ def _load():
             f"tokenpacker_b200: {LIB_PATH} is missing. Build it with `make -C tokenpacker_b200/csrc` "
             "(or `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in SIGNATURES.items():
+    for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

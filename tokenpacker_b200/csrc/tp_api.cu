@@ -9,6 +9,7 @@
 #include <string.h>
 
 #include "../../include/tokenpacker_b200.h"
+#include "../../include/tokenpacker_b200_hd_u8.h"
 #include "tp_gemm.cuh"
 #include "tp_kernels.cuh"
 #include "tp_backward.cuh"
@@ -1612,7 +1613,29 @@ int tp_hd_tile_batch(const tp_hd_image* images_dev, const int32_t* crop_table_de
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const long long blocks = n_crops * (kBlockPx / kHdRows);          // a CTA: kHdRows rows of one crop, one thread per pixel column, 3 channels
   if (blocks > 0x7fffffffll) return TP_ERR_INVALID_ARGUMENT;
-  hd_tile_batch_kernel<<<static_cast<unsigned>(blocks), kBlockPx, 0, stream>>>(reinterpret_cast<const HdImage*>(images_dev), crop_table_dev, n_crops, crops);
+  hd_tile_batch_kernel<<<static_cast<unsigned>(blocks), kBlockPx, 0, stream>>>(reinterpret_cast<const HdImage*>(images_dev), crop_table_dev, n_crops,
+                                                                              HdF32Source{}, crops);
+  TP_CUDA(cudaGetLastError()); ++g_launch_count;
+  return TP_OK;
+}
+
+int tp_hd_preprocess_batch(const tp_hd_image* images_dev, const tp_hd_u8_source* sources_dev, const int32_t* crop_table_dev, int64_t n_crops,
+                           const float* norm_table_dev, int out_dtype, void* crops, void* stream_) {
+  static_assert(sizeof(tp_hd_u8_source) == sizeof(HdU8Image), "tp_hd_u8_source and the kernel's HdU8Image must have the same layout");
+  if (images_dev == nullptr || sources_dev == nullptr || crop_table_dev == nullptr || norm_table_dev == nullptr || crops == nullptr ||
+      n_crops < 0 || (out_dtype != 0 && out_dtype != 1))
+    return TP_ERR_INVALID_ARGUMENT;
+  if (n_crops == 0) return TP_OK;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long blocks = n_crops * (kBlockPx / kHdRows);          // the launch shape of tp_hd_tile_batch
+  if (blocks > 0x7fffffffll) return TP_ERR_INVALID_ARGUMENT;
+  const HdImage* images = reinterpret_cast<const HdImage*>(images_dev);
+  const HdU8Source src{reinterpret_cast<const HdU8Image*>(sources_dev), norm_table_dev};
+  if (out_dtype == 0)
+    hd_tile_batch_kernel<<<static_cast<unsigned>(blocks), kBlockPx, 0, stream>>>(images, crop_table_dev, n_crops, src, static_cast<float*>(crops));
+  else
+    hd_tile_batch_kernel<<<static_cast<unsigned>(blocks), kBlockPx, 0, stream>>>(images, crop_table_dev, n_crops, src,
+                                                                                static_cast<__nv_bfloat16*>(crops));
   TP_CUDA(cudaGetLastError()); ++g_launch_count;
   return TP_OK;
 }

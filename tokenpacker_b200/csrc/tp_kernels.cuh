@@ -388,6 +388,51 @@ struct HdImage {            // mirrors tp_hd_image (include/tokenpacker_b200.h)
   float ty, tx;             // (336 hb) / h_t, (336 wb) / w_t
 };
 
+struct HdU8Image {          // mirrors tp_hd_u8_source (include/tokenpacker_b200_hd_u8.h)
+  const unsigned char* pixels;
+  long long stride_c, stride_y, stride_x;   // element strides of channel, row and column
+};
+
+// Source readers of hd_tile_batch_kernel.  view() binds a reader to one image; View::at(row(y), ch, x) is source pixel (ch, y, x) as
+// the float32 value the tap arithmetic consumes.  The arithmetic is the same for every reader, so equal values give equal bits.
+struct HdF32Source {        // HdImage::image: the normalised float32 [3, h, w] image, contiguous
+  struct View {
+    const float* p;
+    long long plane;
+    int w;
+    __device__ __forceinline__ long long row(int y) const { return static_cast<long long>(y) * w; }
+    __device__ __forceinline__ float at(long long r, int ch, int x) const { return __ldg(p + r + ch * plane + x); }
+  };
+  __device__ __forceinline__ View view(const HdImage& im, int) const { return {im.image, static_cast<long long>(im.h) * im.w, im.w}; }
+};
+
+// Decoded 8-bit pixels at any (channel, row, column) strides, normalised through table[c][u] = (u / 255 - mean[c]) / std[c]
+// (ToTensor + Normalize, train.py:645), which the host computes with the CPU ops torchvision uses.  The 768 floats are staged in
+// shared memory once per CTA: lanes look up different bytes, and constant memory would serialise such divergent reads.
+constexpr int kNormTable = 3 * 256;
+struct HdU8Source {
+  const HdU8Image* sources;   // [n_images], indexed like HdImage
+  const float* table;         // [3][256] float32
+  struct View {
+    const unsigned char* p;
+    long long sc, sy, sx;
+    const float* lut;         // shared memory
+    __device__ __forceinline__ long long row(int y) const { return y * sy; }
+    __device__ __forceinline__ float at(long long r, int ch, int x) const { return lut[ch * 256 + __ldg(p + r + ch * sc + x * sx)]; }
+  };
+  // every thread of the CTA calls this once (it synchronises the CTA)
+  __device__ __forceinline__ View view(const HdImage&, int img) const {
+    __shared__ float lut[kNormTable];
+    for (int i = threadIdx.x; i < kNormTable; i += blockDim.x) lut[i] = __ldg(table + i);
+    __syncthreads();
+    const HdU8Image s = sources[img];
+    return {s.pixels, s.stride_c, s.stride_y, s.stride_x, lut};
+  }
+};
+
+__device__ __forceinline__ void hd_store(float* p, float v) { *p = v; }
+__device__ __forceinline__ void hd_store(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }   // == fp32 crops .to(bfloat16)
+
 __device__ __forceinline__ float hd_canvas_value(const HdImage& im, const float* __restrict__ plane, int Y, int X) {
   if (Y >= im.h_r || X >= im.w_r) return 0.f;
   const LinearTap ty = linear_tap_scaled(Y, im.h, im.sy), tx = linear_tap_scaled(X, im.w, im.sx);
@@ -410,17 +455,19 @@ __device__ __forceinline__ float hd_canvas_value(const HdImage& im, const float*
 constexpr int kHdRows = TP_HD_ROWS;                            // rows per thread; 336 = 42 x 8
 constexpr int kHdUnroll = TP_HD_UNROLL;                        // rows in flight per thread (loads of the next row issue under the math of this one)
 static_assert(kBlockPx % kHdRows == 0, "rows per CTA must divide the crop height");
+// Src: HdF32Source (tp_hd_tile_batch) or HdU8Source (tp_hd_preprocess_batch); Out: float or __nv_bfloat16.
+template <class Src, class Out>
 __global__ void __launch_bounds__(kBlockPx) hd_tile_batch_kernel(const HdImage* __restrict__ images, const int* __restrict__ crop_table,
-                                                                 long long n_crops, float* __restrict__ crops) {
+                                                                 long long n_crops, Src src, Out* __restrict__ crops) {
   constexpr int kRowGroups = kBlockPx / kHdRows;
   const long long crop = blockIdx.x / kRowGroups;
   const int y0 = static_cast<int>(blockIdx.x % kRowGroups) * kHdRows;
   const int x = threadIdx.x;
-  if (crop >= n_crops) return;
+  if (crop >= n_crops) return;                                                     // uniform over the CTA
   const int img = crop_table[crop * 3], ci = crop_table[crop * 3 + 1], cj = crop_table[crop * 3 + 2];
   const HdImage im = images[img];
-  const long long plane_sz = static_cast<long long>(im.h) * im.w;
-  float* out_base = crops + (crop * 3 * kBlockPx + y0) * kBlockPx + x;            // channel stride 336 * 336, row stride 336
+  const typename Src::View s = src.view(im, img);
+  Out* out_base = crops + (crop * 3 * kBlockPx + y0) * kBlockPx + x;              // channel stride 336 * 336, row stride 336
   if (cj >= 0) {
     const int X = cj * kBlockPx + x;
     const bool okx = X < im.w_r;
@@ -430,15 +477,11 @@ __global__ void __launch_bounds__(kBlockPx) hd_tile_batch_kernel(const HdImage* 
       const int Y = ci * kBlockPx + y0 + r;
       const bool ok = okx && Y < im.h_r;
       const LinearTap ty = linear_tap_scaled(ok ? Y : 0, im.h, im.sy);
-      const float* r0 = im.image + static_cast<long long>(ty.i0) * im.w;
-      const float* r1 = im.image + static_cast<long long>(ty.i1) * im.w;
+      const long long r0 = s.row(ty.i0), r1 = s.row(ty.i1);
 #pragma unroll
-      for (int ch = 0; ch < 3; ++ch) {
-        out_base[(static_cast<long long>(ch) * kBlockPx + r) * kBlockPx] =
-            ok ? bilerp(__ldg(r0 + tx.i0), __ldg(r0 + tx.i1), __ldg(r1 + tx.i0), __ldg(r1 + tx.i1), ty, tx) : 0.f;
-        r0 += plane_sz;
-        r1 += plane_sz;
-      }
+      for (int ch = 0; ch < 3; ++ch)
+        hd_store(out_base + (static_cast<long long>(ch) * kBlockPx + r) * kBlockPx,
+                 ok ? bilerp(s.at(r0, ch, tx.i0), s.at(r0, ch, tx.i1), s.at(r1, ch, tx.i0), s.at(r1, ch, tx.i1), ty, tx) : 0.f);
     }
   } else {
     // thumbnail: resized from the PADDED canvas; a canvas tap = the main crops' arithmetic at that canvas pixel (zero outside the content)
@@ -455,22 +498,19 @@ __global__ void __launch_bounds__(kBlockPx) hd_tile_batch_kernel(const HdImage* 
       const LinearTap cy = linear_tap_scaled(ok ? y : 0, ch_h, im.ty);
       const bool oky0 = cy.i0 < im.h_r, oky1 = cy.i1 < im.h_r;
       const LinearTap sy0 = linear_tap_scaled(oky0 ? cy.i0 : 0, im.h, im.sy), sy1 = linear_tap_scaled(oky1 ? cy.i1 : 0, im.h, im.sy);
-      const float* a0 = im.image + static_cast<long long>(sy0.i0) * im.w;   // source rows of canvas row cy.i0
-      const float* a1 = im.image + static_cast<long long>(sy0.i1) * im.w;
-      const float* b0 = im.image + static_cast<long long>(sy1.i0) * im.w;   // ... of canvas row cy.i1
-      const float* b1 = im.image + static_cast<long long>(sy1.i1) * im.w;
+      const long long a0 = s.row(sy0.i0), a1 = s.row(sy0.i1);   // source rows of canvas row cy.i0
+      const long long b0 = s.row(sy1.i0), b1 = s.row(sy1.i1);   // ... of canvas row cy.i1
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) {
         float o = 0.f;
         if (ok) {
-          auto canvas = [&](const float* q0, const float* q1, const LinearTap& sy, bool rowok, const LinearTap& sx, bool colok) {
-            return (rowok && colok) ? bilerp(__ldg(q0 + sx.i0), __ldg(q0 + sx.i1), __ldg(q1 + sx.i0), __ldg(q1 + sx.i1), sy, sx) : 0.f;
+          auto canvas = [&](long long q0, long long q1, const LinearTap& sy, bool rowok, const LinearTap& sx, bool colok) {
+            return (rowok && colok) ? bilerp(s.at(q0, ch, sx.i0), s.at(q0, ch, sx.i1), s.at(q1, ch, sx.i0), s.at(q1, ch, sx.i1), sy, sx) : 0.f;
           };
           o = bilerp(canvas(a0, a1, sy0, oky0, sx0, okx0), canvas(a0, a1, sy0, oky0, sx1, okx1),
                      canvas(b0, b1, sy1, oky1, sx0, okx0), canvas(b0, b1, sy1, oky1, sx1, okx1), cy, cx);
         }
-        out_base[(static_cast<long long>(ch) * kBlockPx + r) * kBlockPx] = o;
-        a0 += plane_sz; a1 += plane_sz; b0 += plane_sz; b1 += plane_sz;
+        hd_store(out_base + (static_cast<long long>(ch) * kBlockPx + r) * kBlockPx, o);
       }
     }
   }

@@ -1,6 +1,7 @@
 """TokenPacker-HD front end: grid selection, crop tiling and slice assembly, host side of the C ABI.
 
 Mirrors the reference seams:
+  * ``Compose([ToTensor(), Normalize(CLIP mean, std)])`` on the decoded image  llava/train/train.py:645 (folded into the tiling launch)
   * ``Image_Patch(image_size=336, patch_num).calculate(h, w)``        llava/patch_divide.py:71-105
   * the inline resize -> pad -> split -> thumbnail block              llava/train/train.py:695-731 (9 pasted copies)
   * the per-image interleaving of crop tokens with ',' / '\\n' rows   llava/model/llava_arch.py:139-155
@@ -107,19 +108,38 @@ def hd_tile_batch(images, patch_num: int = 9, _return_launch: bool = False):
         if not im.is_cuda:
             raise RuntimeError("tokenpacker_b200 has no CPU path: images must be CUDA tensors")
         imgs.append(im.to(torch.float32).contiguous())
-    b = len(imgs)
-    if b == 0:
+    if not imgs:
         raise ValueError("empty batch")
-    device = imgs[0].device
-    hs = (C.c_int64 * b)(*[int(im.shape[1]) for im in imgs])
-    ws = (C.c_int64 * b)(*[int(im.shape[2]) for im in imgs])
-    ptrs = (C.c_void_p * b)(*[im.data_ptr() for im in imgs])
+
+    def launch(tables, _sources, crop_table, n, crops, stream):
+        check(lib.tp_hd_tile_batch(tables, crop_table, n, crops.data_ptr(), stream), "tp_hd_tile_batch")
+
+    crops, hb, wb, (dev, _, table_off, n) = _run_tile_batch(imgs[0].device, [(int(im.shape[1]), int(im.shape[2])) for im in imgs],
+                                                             [im.data_ptr() for im in imgs], None, patch_num, torch.float32, imgs, launch)
+    if _return_launch:
+        # benchmark hook: (device tables, table offset, crop count) so that the kernel can be re-launched and timed on its own
+        return crops, hb, wb, (dev, table_off, n)
+    return crops, hb, wb
+
+
+def _run_tile_batch(device, sizes, image_ptrs, sources, patch_num, out_dtype, keep_alive, launch):
+    """Host side shared by the batched tiling launches: the plan (tp_hd_tile_batch_plan), its tables staged through ONE pinned buffer
+    and ONE asynchronous copy, the crops, and the stream bookkeeping that keeps the source images alive until the kernel has read them.
+
+    sizes: (h, w) per image.  image_ptrs: the float32 images of tp_hd_image, or None.  sources: per image (pixels, stride_c, stride_y,
+    stride_x) of tp_hd_u8_source, staged between the image descriptors and the crop table, or None.  launch(tables, sources, crop_table,
+    n_crops, crops, stream) issues the kernel (device addresses).  Returns (crops, h_block list, w_block list,
+    (device tables, sources offset, crop-table offset, n_crops))."""
+    b = len(sizes)
+    hs = (C.c_int64 * b)(*[h for h, _ in sizes])
+    ws = (C.c_int64 * b)(*[w for _, w in sizes])
+    ptrs = (C.c_void_p * b)(*image_ptrs) if image_ptrs is not None else None
     hb, wb = (C.c_int * b)(), (C.c_int * b)()
     nc = C.c_int64(0)
     check(lib.tp_hd_tile_batch_plan(hs, ws, ptrs, b, int(patch_num), None, None, hb, wb, C.byref(nc)), "tp_hd_tile_batch_plan")
-    # plan tables (image descriptors + crop table) go through ONE pinned staging buffer and ONE asynchronous copy per call
     desc_bytes = C.sizeof(_lib.TpHdImage) * b
-    table_off = (desc_bytes + 15) // 16 * 16
+    src_off = (desc_bytes + 15) // 16 * 16
+    table_off = (src_off + (C.sizeof(_lib.TpHdU8Source) * b if sources is not None else 0) + 15) // 16 * 16
     total_bytes = table_off + max(nc.value, 1) * 12
     st = _staging(device, total_bytes)
     st["event"].synchronize()                     # the previous call's copy has left the pinned buffer
@@ -127,20 +147,93 @@ def hd_tile_batch(images, patch_num: int = 9, _return_launch: bool = False):
     desc = (_lib.TpHdImage * b).from_address(host.data_ptr())
     check(lib.tp_hd_tile_batch_plan(hs, ws, ptrs, b, int(patch_num), desc, C.cast(host.data_ptr() + table_off, C.POINTER(C.c_int32)), hb, wb,
                                     C.byref(nc)), "tp_hd_tile_batch_plan")
+    if sources is not None:
+        rows = (_lib.TpHdU8Source * b).from_address(host.data_ptr() + src_off)
+        for i, s in enumerate(sources):
+            rows[i] = _lib.TpHdU8Source(*s)
     with torch.cuda.device(device):
         dev = st["dev"]
         dev[:total_bytes].copy_(host[:total_bytes], non_blocking=True)
         st["event"].record(torch.cuda.current_stream(device))
-        crops = torch.empty((nc.value, 3, BLOCK, BLOCK), dtype=torch.float32, device=device)
-        stream = torch.cuda.current_stream(device).cuda_stream
-        check(lib.tp_hd_tile_batch(dev.data_ptr(), dev.data_ptr() + table_off, nc.value, crops.data_ptr(), stream), "tp_hd_tile_batch")
+        crops = torch.empty((nc.value, 3, BLOCK, BLOCK), dtype=out_dtype, device=device)
+        stream = torch.cuda.current_stream(device)
+        launch(dev.data_ptr(), dev.data_ptr() + src_off, dev.data_ptr() + table_off, nc.value, crops, stream.cuda_stream)
         # the source images must outlive the asynchronous launch: tie them to the stream
-        for t in imgs:
-            t.record_stream(torch.cuda.current_stream(device))
+        for t in keep_alive:
+            t.record_stream(stream)
+    return crops, list(hb), list(wb), (dev, src_off, table_off, nc.value)
+
+
+# ToTensor() + Normalize(mean, std) of every HD recipe (train.py:645; model_vqa.py:62): the CLIP image statistics
+CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)
+CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
+
+_NORM_TABLE: dict = {}
+
+
+def norm_table() -> torch.Tensor:
+    """float32 [3, 256] on the CPU: entry (c, u) is what ToTensor + Normalize make of byte u in channel c.
+
+    Computed with the CPU ops torchvision runs (uint8 -> float, div(255), then sub(mean) and div(std) per channel), so every entry
+    has torchvision's bits.  Not computed on the device: ATen's CUDA kernels may divide by a scalar as a multiplication by its
+    reciprocal, which can differ in the last bit."""
+    u = torch.arange(256, dtype=torch.uint8)
+    mean = torch.tensor(CLIP_MEAN, dtype=torch.float32)
+    std = torch.tensor(CLIP_STD, dtype=torch.float32)
+    return (u.float().div(255) - mean[:, None]) / std[:, None]
+
+
+def _norm_table_on(device) -> torch.Tensor:
+    key = str(device)
+    t = _NORM_TABLE.get(key)
+    if t is None:
+        t = _NORM_TABLE[key] = norm_table().to(device)
+    return t
+
+
+def hd_preprocess_batch(images, patch_num: int = 9, dtype=torch.float32, layout: str = "HWC", _return_launch: bool = False):
+    """ToTensor + Normalize (train.py:645) and the tiling block (train.py:695-731) for a batch of DECODED 8-bit images, in one launch.
+
+    images: sequence of uint8 CUDA tensors, [h, w, 3] for layout "HWC" (np.array(pil_image), what the reference decodes) or [3, h, w]
+    for "CHW" (torchvision.io.decode_image); sizes may differ, and views are read through their strides, not copied.
+    dtype: torch.float32, or torch.bfloat16 (the tower's dtype; equal to the float32 crops .to(torch.bfloat16), bit for bit).
+    Returns (crops [sum_i n_crops_i, 3, 336, 336] in dtype, h_block list, w_block list) in the reference's crop order.  The float32
+    crops have exactly the bits hd_tile_batch gives for the same images normalised on the host (norm_table)."""
+    if dtype not in (torch.float32, torch.bfloat16):
+        raise ValueError(f"dtype must be torch.float32 or torch.bfloat16, not {dtype}")
+    if layout not in ("HWC", "CHW"):
+        raise ValueError(f'layout must be "HWC" or "CHW", not {layout!r}')
+    images = list(images)
+    if not images:
+        raise ValueError("empty batch")
+    cdim = 2 if layout == "HWC" else 0
+    for im in images:
+        if im.dtype != torch.uint8:
+            raise TypeError(f"images must be uint8 (decoded pixels), not {im.dtype}")
+        if im.dim() != 3 or im.shape[cdim] != 3:
+            raise ValueError(f"each image is {'[h,w,3]' if layout == 'HWC' else '[3,h,w]'} for layout {layout!r}, got {tuple(im.shape)}")
+        if not im.is_cuda:
+            raise RuntimeError("tokenpacker_b200 has no CPU path: images must be CUDA tensors (move pinned uint8 images with .cuda(non_blocking=True))")
+    device = images[0].device
+    if any(im.device != device for im in images):
+        raise ValueError("all images must be on one device")
+    if layout == "HWC":
+        sizes = [(int(im.shape[0]), int(im.shape[1])) for im in images]
+        sources = [(im.data_ptr(), im.stride(2), im.stride(0), im.stride(1)) for im in images]
+    else:
+        sizes = [(int(im.shape[1]), int(im.shape[2])) for im in images]
+        sources = [(im.data_ptr(), im.stride(0), im.stride(1), im.stride(2)) for im in images]
+    table = _norm_table_on(device)
+    out_dtype = 0 if dtype == torch.float32 else 1
+
+    def launch(tables, srcs, crop_table, n, crops, stream):
+        check(lib.tp_hd_preprocess_batch(tables, srcs, crop_table, n, table.data_ptr(), out_dtype, crops.data_ptr(), stream), "tp_hd_preprocess_batch")
+
+    crops, hb, wb, plan = _run_tile_batch(device, sizes, None, sources, patch_num, dtype, images, launch)
     if _return_launch:
-        # benchmark hook: (device tables, table offset, crop count) so that the kernel can be re-launched and timed on its own
-        return crops, list(hb), list(wb), (dev, table_off, nc.value)
-    return crops, list(hb), list(wb)
+        # benchmark hook: (device tables, sources offset, crop-table offset, crop count, device norm table)
+        return crops, hb, wb, plan + (table,)
+    return crops, hb, wb
 
 
 def hd_seq_len(hb: int, wb: int, m: int) -> int:
