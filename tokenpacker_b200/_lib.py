@@ -1,7 +1,7 @@
 """ctypes binding of libtokenpacker_b200.so — the thin seam between the Python host code and the C-ABI CUDA library.
 
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
-Signatures mirror include/tokenpacker_b200.h and include/tokenpacker_b200_hd_u8.h one to one.
+Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h and include/tokenpacker_b200_input_grad.h one to one.
 """
 from __future__ import annotations
 
@@ -109,6 +109,12 @@ HD_U8_SIGNATURES = {
     "tp_hd_preprocess_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
 }
 
+# the same for include/tokenpacker_b200_input_grad.h (gradients w.r.t. the CLIP features in the training path)
+INPUT_GRAD_SIGNATURES = {
+    "tp_backward_inputs": (C.c_int, [C.POINTER(TpWeights), C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                     C.c_void_p, C.POINTER(TpWeights), C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+}
+
 
 def _load():
     if not os.path.exists(LIB_PATH):
@@ -116,7 +122,7 @@ def _load():
             f"tokenpacker_b200: {LIB_PATH} is missing. Build it with `make -C tokenpacker_b200/csrc` "
             "(or `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES}.items():
+    for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

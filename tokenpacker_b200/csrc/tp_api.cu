@@ -10,6 +10,7 @@
 
 #include "../../include/tokenpacker_b200.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
+#include "../../include/tokenpacker_b200_input_grad.h"
 #include "tp_gemm.cuh"
 #include "tp_kernels.cuh"
 #include "tp_backward.cuh"

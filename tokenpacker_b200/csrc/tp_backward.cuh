@@ -1,6 +1,7 @@
 // Kernels of the projector's backward pass that are not GEMMs: GELU forward/backward as elementwise passes, LayerNorm apply /
-// backward, window-attention backward, deterministic column sums (bias gradients), and a plain transpose (weights for the
-// dgrad GEMMs; activations only in the small-hidden wgrad fallback).  All HBM-bound, 16-byte vector accesses.
+// backward, window-attention backward, deterministic column sums (bias gradients), a plain transpose (weights for the
+// dgrad GEMMs; activations only in the small-hidden wgrad fallback), and the point-query stencil backwards (the gradient w.r.t.
+// the CLIP feature x0, when asked for).  All HBM-bound, 16-byte vector accesses.
 // The GEMMs of the backward run on the forward's wgmma kernels: dgrad (dX = dY . W) takes a transposed copy of the weight as
 // its K-major B operand; wgrad (dW = dY^T . X) uses the TN form, reading both activations in place as MN-major tiles.
 #pragma once
@@ -511,6 +512,48 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
   o.x = pack_bf16x2(acc.x * alpha, acc.y * alpha);
   o.y = pack_bf16x2(acc.z * alpha, acc.w * alpha);
   *reinterpret_cast<uint2*>(out + i) = o;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Point-query stencil backwards (the transpose of point_query_kernel): dx0 [n_tokens, 1024] from dq [N g^2, 1024].
+// With align_corners=False and no edge clamping for any divisor s of 24, every fine token is a tap of at most one query, its own
+// window's, so the transpose is a gather: per fine token (r, c) of crop n, with m = (r / s) g + c / s,
+//   odd s:  dx0 = dq[n, m] at the window's centre token, 0 elsewhere;
+//   even s: dx0 = bf16(0.25 float(dq[n, m])) on the centre 2x2, 0 elsewhere (s = 2: every token).
+// That is the reference's upsample_bilinear2d backward (weights 0.5 x 0.5, fp32) followed by the bf16 rounding of .float()'s
+// backward; 0.25 x is exact in fp32, so the bits match given the same dq.  Writes every element, zeros included.
+// One thread per 8 channels of one fine token.
+// ------------------------------------------------------------------------------------------------
+template <int S>
+__global__ void __launch_bounds__(256) point_query_bwd_kernel(const __nv_bfloat16* __restrict__ dq, __nv_bfloat16* __restrict__ dx0,
+                                                              long long n_tokens) {
+  constexpr int G = kGrid / S;
+  constexpr int M = G * G;
+  constexpr int kLo = (S % 2 == 1) ? (S - 1) / 2 : S / 2 - 1;     // first tap row / column inside the window
+  constexpr int kHi = (S % 2 == 1) ? kLo : kLo + 1;               // last
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long tok = idx >> 7;            // 128 vectors of 8 channels per token
+  const int vec = static_cast<int>(idx & 127);
+  if (tok >= n_tokens) return;
+  const long long n = tok / kTokens;
+  const int t = static_cast<int>(tok - n * kTokens);
+  const int r = t / kGrid, c = t - r * kGrid;
+  const int hb = r / S, wb = c / S;
+  const int ri = r - hb * S, ci = c - wb * S;
+  uint4 out = make_uint4(0u, 0u, 0u, 0u);
+  if (ri >= kLo && ri <= kHi && ci >= kLo && ci <= kHi) {
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(dq + (n * M + hb * G + wb) * kC + vec * 8));
+    if (S % 2 == 1) {
+      out = v;
+    } else {
+      float f[8];
+      unpack8(v, f);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) f[i] = __fmul_rn(0.25f, f[i]);
+      out = pack8(f);
+    }
+  }
+  *reinterpret_cast<uint4*>(dx0 + tok * kC + vec * 8) = out;
 }
 
 }  // namespace tp

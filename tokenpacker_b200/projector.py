@@ -40,7 +40,8 @@ def _two_layer(in_dim: int, mid: int, out: int) -> nn.Sequential:
 
 
 class _ProjectorFunction(torch.autograd.Function):
-    """autograd bridge: forward = tp_forward_train (keeps intermediates), backward = tp_backward (parameter gradients)."""
+    """autograd bridge: forward = tp_forward_train (keeps intermediates), backward = tp_backward (parameter gradients), or
+    tp_backward_inputs when x0b / xmb need a gradient too (``TokenPackerB200.input_grad``)."""
 
     @staticmethod
     def forward(ctx, module, x0b, s0, xmb, sm, *params):
@@ -65,6 +66,7 @@ class _ProjectorFunction(torch.autograd.Function):
                                    module.hidden_size, out.data_ptr(), saved.data_ptr(), nbytes, stream), "tp_forward_train")
         ctx.module = module
         ctx.saved = saved
+        ctx.packed = packed if ctx.needs_input_grad[3] else None     # dxm reads [W_k0; W_v0] from it; ~80 MB at hidden 4096, else dropped
         ctx.xm = xmb if xmb.is_contiguous() else xmb.contiguous()
         ctx.weights_bf16 = bf                                # the parameters this forward read (bf16; aliases of the live ones when they are bf16)
         ctx.param_meta = [(p.dtype, p.requires_grad) for p in params]
@@ -80,14 +82,24 @@ class _ProjectorFunction(torch.autograd.Function):
         grads = [torch.empty_like(w) for w in ctx.weights_bf16]
         w_struct = _lib.TpWeights(*[t.data_ptr() for t in ctx.weights_bf16])
         g_struct = _lib.TpWeights(*[t.data_ptr() for t in grads])
+        need_x0, need_xm = ctx.needs_input_grad[1], ctx.needs_input_grad[3]
+        d_x0 = d_xm = None
         with torch.cuda.device(device):
             ws_bytes = lib.tp_backward_workspace_bytes(n, module.scale_factor, module.hidden_size)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
             stream = torch.cuda.current_stream(device).cuda_stream
-            check(lib.tp_backward(C.byref(w_struct), ctx.xm.data_ptr(), ctx.xm.stride(0), n, module.scale_factor, module.hidden_size,
-                                  g.data_ptr(), ctx.saved.data_ptr(), C.byref(g_struct), ws.data_ptr(), ws_bytes, stream), "tp_backward")
+            if need_x0 or need_xm:
+                d_x0 = torch.empty((n, 576, 1024), dtype=torch.bfloat16, device=device) if need_x0 else None     # every element written
+                d_xm = torch.empty((n, 576, 4096), dtype=torch.bfloat16, device=device) if need_xm else None
+                check(lib.tp_backward_inputs(C.byref(w_struct), ctx.packed.data_ptr() if need_xm else None, ctx.xm.data_ptr(),
+                                             ctx.xm.stride(0), n, module.scale_factor, module.hidden_size, g.data_ptr(), ctx.saved.data_ptr(),
+                                             C.byref(g_struct), d_x0.data_ptr() if need_x0 else None,
+                                             d_xm.data_ptr() if need_xm else None, ws.data_ptr(), ws_bytes, stream), "tp_backward_inputs")
+            else:
+                check(lib.tp_backward(C.byref(w_struct), ctx.xm.data_ptr(), ctx.xm.stride(0), n, module.scale_factor, module.hidden_size,
+                                      g.data_ptr(), ctx.saved.data_ptr(), C.byref(g_struct), ws.data_ptr(), ws_bytes, stream), "tp_backward")
         out = [gr.to(dt) if need else None for gr, (dt, need) in zip(grads, ctx.param_meta)]
-        return (None, None, None, None, None) + tuple(out)
+        return (None, d_x0, None, d_xm, None) + tuple(out)
 
 
 class _PackedScatterFunction(torch.autograd.Function):
@@ -162,6 +174,11 @@ class TokenPackerB200(nn.Module):
         self._keepalive = None
         self._param_list = None
         self._warned_dtype = False
+        # Gradients w.r.t. the CLIP features (unfrozen vision tower, LoRA / adapters on CLIP, attribution on the image features):
+        # off by default, so that features left with requires_grad by accident keep failing loudly instead of silently costing the
+        # xm gradient (a GEMM as large as the forward's largest, and [N,576,4096] bf16 of memory).  Set to True to have forward()
+        # and forward_packed() carry gradients to feat / feat_multi.  Not a constructor argument and not in the state_dict.
+        self.input_grad = False
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
 
     @staticmethod
@@ -232,7 +249,7 @@ class TokenPackerB200(nn.Module):
         t = t.contiguous()
         return t, t.stride(0)
 
-    def _check_inputs(self, x, attn_mask):
+    def _check_inputs(self, x, attn_mask, differentiable: bool = True):
         if attn_mask is not None:
             raise NotImplementedError("attn_mask must be None (the reference's sole caller passes none, llava_arch.py:97)")
         if not isinstance(x, (tuple, list)) or len(x) != 2:
@@ -248,10 +265,14 @@ class TokenPackerB200(nn.Module):
             warnings.warn("tokenpacker_b200 computes with bf16 storage and fp32 accumulation: fp16 / fp32 inputs and parameters are cast to "
                           "bf16 at the boundary and the result is cast back (every released TokenPacker recipe runs bf16; an fp16 or "
                           "fp32 module gets bf16-precision results)", stacklevel=3)
-        if torch.is_grad_enabled() and (x0.requires_grad or xm.requires_grad):
-            raise NotImplementedError("gradients w.r.t. the CLIP features are not implemented (the vision tower is frozen in every "
-                                      "released TokenPacker recipe): detach the features or run under torch.no_grad()")
+        if torch.is_grad_enabled() and (x0.requires_grad or xm.requires_grad) and not (self.input_grad and differentiable):
+            raise NotImplementedError("gradients w.r.t. the CLIP features are off by default (the vision tower is frozen in every "
+                                      "released TokenPacker recipe): set `projector.input_grad = True` to have forward() / forward_packed() "
+                                      "produce them, or detach the features or run under torch.no_grad()")
         return x0, xm
+
+    def _inputs_need_grad(self, x0, xm) -> bool:
+        return self.input_grad and torch.is_grad_enabled() and (x0.requires_grad or xm.requires_grad)
 
     def forward(self, x, attn_mask=None):
         x0, xm = self._check_inputs(x, attn_mask)
@@ -263,8 +284,9 @@ class TokenPackerB200(nn.Module):
         with torch.cuda.device(device):
             x0b, s0 = self._as_crop_strided(x0.to(torch.bfloat16), 1024)
             xmb, sm = self._as_crop_strided(xm.to(torch.bfloat16), 4096)
-            if torch.is_grad_enabled() and any(p.requires_grad for p in self._raw_params()):
-                # training: same output, intermediates kept, gradients for every parameter (tp_forward_train / tp_backward)
+            if (torch.is_grad_enabled() and any(p.requires_grad for p in self._raw_params())) or self._inputs_need_grad(x0, xm):
+                # training: same output, intermediates kept, gradients for every parameter (tp_forward_train / tp_backward) and, with
+                # input_grad, for the features that require one (tp_backward_inputs)
                 out = _ProjectorFunction.apply(self, x0b, s0, xmb, sm, *self._raw_params())
             else:
                 out = torch.empty((n, self.num_queries, self.hidden_size), dtype=torch.bfloat16, device=device)
@@ -332,7 +354,7 @@ class TokenPackerB200(nn.Module):
         = M + 1: the packed HD rows of llava_arch.py:139-155 directly (separator rows are the caller's).  Asynchronous; a cross-rank
         barrier must follow.  Inference only."""
         self._require_inference("forward_into_peers")
-        x0, xm = self._check_inputs(x, None)
+        x0, xm = self._check_inputs(x, None, differentiable=False)
         device = x0.device
         with torch.cuda.device(device):
             x0b, s0 = self._as_crop_strided(x0.to(torch.bfloat16), 1024)
@@ -397,7 +419,7 @@ class TokenPackerB200(nn.Module):
         crop_rows = self.num_queries + 1
         assert total == plan.n_crops * crop_rows      # one separator row per crop: the uniform stride the kernel relies on
         training = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or sep_row.requires_grad
-                                                or ret_row.requires_grad)
+                                                or ret_row.requires_grad or self._inputs_need_grad(x0, xm))
         with torch.cuda.device(device):
             if training:
                 feats = self.forward((x0, xm)).to(torch.bfloat16)
