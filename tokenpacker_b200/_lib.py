@@ -9,9 +9,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# TOKENPACKER_B200_LIB_OVERRIDE: load another BUILD of the same library (A/B experiments with -D variants); it must export
-# every symbol of the header like the default one.  Unset in normal use.
-LIB_PATH = os.environ.get("TOKENPACKER_B200_LIB_OVERRIDE") or os.path.join(_HERE, "libtokenpacker_b200.so")
+LIB_PATH = os.path.join(_HERE, "libtokenpacker_b200.so")
 
 TP_OK = 0
 TP_ERR_INVALID_ARGUMENT = 1

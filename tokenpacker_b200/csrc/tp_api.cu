@@ -58,49 +58,43 @@ EncodeTiledFn encode_tiled_fn() {
   return fn;
 }
 
-// bf16 matrix [rows, cols] with row stride ld (elements); box = 64 columns x box_rows rows, 128-byte swizzle.
-int make_map_2d(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld, int box_rows, int box_cols = kBlockK) {
+// bf16 tensor of `rank` dimensions, innermost first: extents `dims`, byte strides `strides` of dimensions 1 .. rank-1, boxes of
+// `box` elements.  Every box is 64 columns wide (128 bytes: one row of the 128-byte swizzle the operand tiles and output slabs use).
+static_assert(kSlabCols == kBlockK, "output slabs and operand tiles share the 64-column, 128-byte swizzle rows");
+int encode_bf16_map(CUtensorMap* map, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides, const cuuint32_t* box) {
   EncodeTiledFn fn = encode_tiled_fn();
   if (fn == nullptr) {
     snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "cuTensorMapEncodeTiled entry point not found");
     return TP_ERR_CUDA;
   }
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * 2) % 16 != 0) return TP_ERR_INVALID_ARGUMENT;
-  cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * 2};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0) return TP_ERR_INVALID_ARGUMENT;
+  for (int i = 0; i < rank - 1; ++i)
+    if (strides[i] % 16 != 0) return TP_ERR_INVALID_ARGUMENT;
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, static_cast<cuuint32_t>(rank), const_cast<void*>(ptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "cuTensorMapEncodeTiled(2d) failed: %d", static_cast<int>(r));
+    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "cuTensorMapEncodeTiled(%dd) failed: %d", rank, static_cast<int>(r));
     return TP_ERR_CUDA;
   }
   return TP_OK;
 }
 
-// bf16 tensor [segs, seg_rows, cols] with row stride ld and segment stride seg_stride (elements); box 64 x 64 x 1.
+// bf16 matrix [rows, cols] with row stride ld (elements); box = 64 columns x box_rows rows.
+int make_map_2d(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld, int box_rows) {
+  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * 2};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kBlockK), static_cast<cuuint32_t>(box_rows)};
+  return encode_bf16_map(map, ptr, 2, dims, strides, box);
+}
+
+// bf16 tensor [segs, seg_rows, cols] with row stride ld and segment stride seg_stride (elements); box 64 x box_rows x box_segs.
 int make_map_3d(CUtensorMap* map, const void* ptr, long long segs, long long seg_rows, long long cols, long long ld,
-                long long seg_stride, int box_rows = 64, int box_cols = kBlockK, bool swizzle = true, int box_segs = 1) {
-  EncodeTiledFn fn = encode_tiled_fn();
-  if (fn == nullptr) {
-    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "cuTensorMapEncodeTiled entry point not found");
-    return TP_ERR_CUDA;
-  }
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * 2) % 16 != 0 || (seg_stride * 2) % 16 != 0) return TP_ERR_INVALID_ARGUMENT;
-  cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(seg_rows), static_cast<cuuint64_t>(segs)};
-  cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * 2, static_cast<cuuint64_t>(seg_stride) * 2};
-  cuuint32_t box[3] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows), static_cast<cuuint32_t>(box_segs)};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, !swizzle ? CU_TENSOR_MAP_SWIZZLE_NONE : (box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B), CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "cuTensorMapEncodeTiled(3d) failed: %d", static_cast<int>(r));
-    return TP_ERR_CUDA;
-  }
-  return TP_OK;
+                long long seg_stride, int box_rows = 64, int box_segs = 1) {
+  const cuuint64_t dims[3] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(seg_rows), static_cast<cuuint64_t>(segs)};
+  const cuuint64_t strides[2] = {static_cast<cuuint64_t>(ld) * 2, static_cast<cuuint64_t>(seg_stride) * 2};
+  const cuuint32_t box[3] = {static_cast<cuuint32_t>(kBlockK), static_cast<cuuint32_t>(box_rows), static_cast<cuuint32_t>(box_segs)};
+  return encode_bf16_map(map, ptr, 3, dims, strides, box);
 }
 
 // Window-major destination of a raster-ordered [crops * 576, cols] bf16 matrix (scale factor s, g = 24 / s): dims
@@ -108,28 +102,15 @@ int make_map_3d(CUtensorMap* map, const void* ptr, long long segs, long long seg
 // (box_tokens / s) x 1 = box_tokens consecutive tokens of one token row (hi has extent 1 in the box, so the box is traversed
 // wi-then-wb: raster order).  box_tokens in {8, 16, 24}: stores never stick out of the tensor (that faults), so each piece of a
 // slab uses the map of exactly its size.
-int make_map_wm(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld, int s, int box_tokens, bool swizzle = true) {
-  EncodeTiledFn fn = encode_tiled_fn();
-  if (fn == nullptr) {
-    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "cuTensorMapEncodeTiled entry point not found");
-    return TP_ERR_CUDA;
-  }
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * 2) % 16 != 0 || rows % 576 != 0 || (s != 2 && s != 4 && s != 8)) return TP_ERR_INVALID_ARGUMENT;
+int make_map_wm(CUtensorMap* map, const void* ptr, long long rows, long long cols, long long ld, int s, int box_tokens) {
+  if (rows % 576 != 0 || (s != 2 && s != 4 && s != 8) || box_tokens % s != 0 || box_tokens > 24) return TP_ERR_INVALID_ARGUMENT;
   const int g = 24 / s;
-  cuuint64_t dims[5] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(s), static_cast<cuuint64_t>(s), static_cast<cuuint64_t>(g),
-                        static_cast<cuuint64_t>(rows / 576 * g)};
+  const cuuint64_t dims[5] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(s), static_cast<cuuint64_t>(s), static_cast<cuuint64_t>(g),
+                              static_cast<cuuint64_t>(rows / 576 * g)};
   const cuuint64_t row_b = static_cast<cuuint64_t>(ld) * 2;
-  cuuint64_t strides[4] = {row_b, row_b * s, row_b * s * s, row_b * s * s * g};
-  if (box_tokens % s != 0 || box_tokens > 24) return TP_ERR_INVALID_ARGUMENT;
-  cuuint32_t box[5] = {static_cast<cuuint32_t>(kSlabCols), static_cast<cuuint32_t>(s), 1, static_cast<cuuint32_t>(box_tokens / s), 1};
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  !swizzle ? CU_TENSOR_MAP_SWIZZLE_NONE : (kSlabCols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B), CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "cuTensorMapEncodeTiled(5d) failed: %d", static_cast<int>(r));
-    return TP_ERR_CUDA;
-  }
-  return TP_OK;
+  const cuuint64_t strides[4] = {row_b, row_b * s, row_b * s * s, row_b * s * s * g};
+  const cuuint32_t box[5] = {static_cast<cuuint32_t>(kSlabCols), static_cast<cuuint32_t>(s), 1, static_cast<cuuint32_t>(box_tokens / s), 1};
+  return encode_bf16_map(map, ptr, 5, dims, strides, box);
 }
 
 struct DeviceInfo {
@@ -172,8 +153,7 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  static const bool no_pdl = getenv("TP_NO_PDL") != nullptr;   // debugging aid: plain stream serialization
-  cfg.numAttrs = no_pdl ? 0 : 1;
+  cfg.numAttrs = 1;
   ++g_launch_count;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
@@ -249,22 +229,6 @@ int launch_gemm_t(const GemmItem& it, int sms, cudaStream_t stream) {
   return TP_OK;
 }
 
-// Up to kMaxGroup independent problems in ONE launch of the CTA-pair kernel.
-// A tile schedule for a chained launch: segments (item, first row block, row blocks) in issue order; see TileSeg.
-struct SegPlan {
-  int n = 0;
-  int prob[kMaxSegs], m_lo[kMaxSegs], m_cnt[kMaxSegs];
-  bool add(int p, long long lo, long long hi, long long blocks) {
-    if (lo < 0) lo = 0;
-    if (hi > blocks) hi = blocks;
-    if (hi <= lo) return true;
-    if (n == kMaxSegs) return false;
-    prob[n] = p; m_lo[n] = static_cast<int>(lo); m_cnt[n] = static_cast<int>(hi - lo);
-    ++n;
-    return true;
-  }
-};
-
 // Everything a launch of the pair kernel needs, as built from a list of items: kept by the forward plan cache below (encoding
 // ~100 tensor maps per call costs more host time than the whole 32-crop forward takes on the GPU).
 struct BuiltLaunch {
@@ -273,8 +237,9 @@ struct BuiltLaunch {
   int grid;
 };
 
+// Up to kMaxGroup independent problems in ONE launch of the CTA-pair kernel.
 int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream_t stream, const FrontWork* front = nullptr,
-                           const SegPlan* plan = nullptr, BuiltLaunch* built = nullptr) {
+                           BuiltLaunch* built = nullptr) {
   using Cfg = Gemm2Config;
   GemmGroup g;
   memset(&g, 0, sizeof(g));
@@ -338,19 +303,13 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
     // uniformly strided segments (the HD packed layout) stay on the TMA path through a 3-D (cols, row in segment, segment) map
     p.use_tma_store = (it.ep.seg_row_offset == nullptr && !it.ep.out_f32) ? 1 : 0;
     const bool c_segmented = p.use_tma_store && it.ep.seg_stride != 0 && it.ep.seg_stride != it.ep.seg_len;
-    // A/B aid (read per call): TP_SEG_NOSWIZZLE=1 builds the clipped-box maps (segmented rows, window-major rows) without
-    // swizzle; the epilogue then writes plain slab rows for those problems (bank-conflicted, but only their stores are affected)
-    const char* nsw_env = getenv("TP_SEG_NOSWIZZLE");
-    const bool noswz = nsw_env != nullptr && atoi(nsw_env) != 0;
     if (it.ep.wm_s != 0) {
       if (!p.use_tma_store || c_segmented || it.n_peers > 0) return TP_ERR_INVALID_ARGUMENT;
       p.c_wm_s = it.ep.wm_s;
-      p.c_noswz = noswz ? 1 : 0;
-      TP_TRY(make_map_wm(&p.tmap_c, it.ep.c, it.M, it.N, it.ep.ldc, it.ep.wm_s, 8, !noswz));
-      TP_TRY(make_map_wm(&p.tmap_cx[0], it.ep.c, it.M, it.N, it.ep.ldc, it.ep.wm_s, 16, !noswz));
-      TP_TRY(make_map_wm(&p.tmap_cx[1], it.ep.c, it.M, it.N, it.ep.ldc, it.ep.wm_s, 24, !noswz));
+      TP_TRY(make_map_wm(&p.tmap_c, it.ep.c, it.M, it.N, it.ep.ldc, it.ep.wm_s, 8));
+      TP_TRY(make_map_wm(&p.tmap_cx[0], it.ep.c, it.M, it.N, it.ep.ldc, it.ep.wm_s, 16));
+      TP_TRY(make_map_wm(&p.tmap_cx[1], it.ep.c, it.M, it.N, it.ep.ldc, it.ep.wm_s, 24));
     } else if (c_segmented) {
-      p.c_noswz = noswz ? 1 : 0;
       if (it.ep.seg_len <= 0 || it.M % it.ep.seg_len != 0 || it.ep.seg_stride < it.ep.seg_len) return TP_ERR_INVALID_ARGUMENT;
       p.c_seg_len = it.ep.seg_len;
       p.c_unit = 128;
@@ -360,17 +319,16 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
         int rows = p.c_unit << lvl;
         if (rows > kBlockM || rows > it.ep.seg_len) rows = p.c_unit;  // level never used (pieces are at most min(seg_len, 128) rows)
         TP_TRY(make_map_3d(lvl == 0 ? &p.tmap_c : &p.tmap_cx[lvl - 1], it.ep.c, it.M / it.ep.seg_len, it.ep.seg_len, it.N, it.ep.ldc,
-                           it.ep.seg_stride * it.ep.ldc, rows, kSlabCols, !noswz));
+                           it.ep.seg_stride * it.ep.ldc, rows));
       }
     } else {
-      TP_TRY(make_map_2d(&p.tmap_c, it.ep.c, it.M, it.N, it.ep.ldc, kBlockM, kSlabCols));
+      TP_TRY(make_map_2d(&p.tmap_c, it.ep.c, it.M, it.N, it.ep.ldc, kBlockM));
     }
     if (it.ep.dual) {
-      // pre-activation copy: plain TMA-store output only, and the two staging buffers of a half must exist (z and GELU(z) slabs side by side)
-      if (!p.use_tma_store || c_segmented || it.ep.wm_s != 0 || it.n_peers > 0 || !it.ep.gelu || it.c_pre == nullptr || Cfg::kOutBufs != 2 ||
-          kSlabCols != 64 || it.k_splits > 1)
+      // pre-activation copy: plain TMA-store output only (z and GELU(z) slabs side by side in the half's two staging buffers)
+      if (!p.use_tma_store || c_segmented || it.ep.wm_s != 0 || it.n_peers > 0 || !it.ep.gelu || it.c_pre == nullptr || it.k_splits > 1)
         return TP_ERR_INVALID_ARGUMENT;
-      TP_TRY(make_map_2d(&p.tmap_cx[0], it.c_pre, it.M, it.N, it.ld_pre, kBlockM, kSlabCols));
+      TP_TRY(make_map_2d(&p.tmap_cx[0], it.c_pre, it.M, it.N, it.ld_pre, kBlockM));
     }
     p.M = static_cast<int>(it.M);
     p.N = static_cast<int>(it.N);
@@ -400,21 +358,6 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
   if (total > 0x7fffffffll) return TP_ERR_INVALID_ARGUMENT;
   g.total_tiles = static_cast<int>(total);
   if (front != nullptr) g.front = *front;
-  if (plan != nullptr && plan->n > 0) {
-    // the schedule must cover every row block of every problem exactly once (else fall back to stage order)
-    long long covered[kMaxGroup] = {0};
-    int t0 = 0;
-    bool ok = true;
-    for (int i = 0; i < plan->n && ok; ++i) {
-      const GemmProblem& pp = g.p[plan->prob[i]];
-      if (pp.k_splits != 1) ok = false;
-      g.segs[i] = TileSeg{plan->prob[i], plan->m_lo[i], t0, plan->m_cnt[i] * pp.num_n_blocks};
-      t0 += g.segs[i].n_tiles;
-      covered[plan->prob[i]] += plan->m_cnt[i];
-    }
-    for (int i = 0; i < count && ok; ++i) ok = covered[i] * g.p[i].num_n_blocks == g.p[i].num_tiles;
-    g.n_segs = (ok && t0 == g.total_tiles) ? plan->n : 0;
-  }
   PeerStores peers;
   memset(&peers, 0, sizeof(peers));
   int peer_item = -1;
@@ -462,20 +405,19 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
         for (int lvl = 0; lvl < kBoxLevels; ++lvl) {
           int rows = p0.c_unit << lvl;
           if (rows > kBlockM || rows > it0.ep.seg_len) rows = p0.c_unit;
-          TP_TRY(make_map_3d(&peers.m[p][lvl], dst[p], n_segs, it0.ep.seg_len, it0.N, it0.ep.ldc,
-                             it0.ep.seg_stride * it0.ep.ldc, rows, kSlabCols, p0.c_noswz == 0));
+          TP_TRY(make_map_3d(&peers.m[p][lvl], dst[p], n_segs, it0.ep.seg_len, it0.N, it0.ep.ldc, it0.ep.seg_stride * it0.ep.ldc, rows));
         }
         for (int k = 1; k <= kWholeLevels; ++k) {
           // k whole segments; a level that can never be used (k segments do not fit a slab, or there are fewer segments) repeats k = 1
           const int kk = (whole && k * it0.ep.seg_len <= kBlockM && k <= n_segs) ? k : 1;
           if (whole)
             TP_TRY(make_map_3d(&peers.m[p][kBoxLevels + k - 1], dst[p], n_segs, it0.ep.seg_len, it0.N, it0.ep.ldc,
-                               it0.ep.seg_stride * it0.ep.ldc, it0.ep.seg_len, kSlabCols, p0.c_noswz == 0, kk));
+                               it0.ep.seg_stride * it0.ep.ldc, it0.ep.seg_len, kk));
           else
             peers.m[p][kBoxLevels + k - 1] = peers.m[p][0];
         }
       } else {
-        TP_TRY(make_map_2d(&peers.m[p][0], dst[p], it0.M, it0.N, it0.ep.ldc, kBlockM, kSlabCols));
+        TP_TRY(make_map_2d(&peers.m[p][0], dst[p], it0.M, it0.N, it0.ep.ldc, kBlockM));
       }
     }
     peers.count = n_dst;
@@ -603,7 +545,7 @@ bool chain_feasible(const GemmItem* items, int count, int sms, bool by_cost = tr
 }
 
 int launch_chain(GemmItem* items, int count, int* flags, long long flag_capacity, const FrontWork* front, int sms, cudaStream_t stream,
-                 const SegPlan* plan = nullptr, BuiltLaunch* built = nullptr) {
+                 BuiltLaunch* built = nullptr) {
   if (count <= 0 || count > kMaxGroup) return TP_ERR_INVALID_ARGUMENT;
   for (int i = 0; i < count; ++i) {
     const int deps[3] = {items[i].dep, items[i].dep2, items[i].dep3};
@@ -668,7 +610,7 @@ int launch_chain(GemmItem* items, int count, int* flags, long long flag_capacity
         it.dep_target = gemm_target(d);
       }
     }
-    return launch_gemm_pair_group(items, count, sms, stream, front != nullptr ? &fw : nullptr, plan, built);
+    return launch_gemm_pair_group(items, count, sms, stream, front != nullptr ? &fw : nullptr, built);
   }
   for (int i = 0; i < count; ++i)
     if (items[i].kind == 1 || items[i].ep.wm_s != 0) return TP_ERR_INVALID_ARGUMENT;      // fused-attention items exist only inside a chain
@@ -965,11 +907,12 @@ size_t tp_workspace_bytes(int64_t n_crops, int scale_factor, int hidden) {
 namespace {
 // Plan cache of the single-launch forward: the launch is a pure function of these values (tensor maps depend on addresses and shapes
 // only), so a call that repeats them — a serving loop, the chunks of tp_forward_host, the ranks of a sharded HD batch — skips the
-// ~100 cuTensorMapEncodeTiled calls and replays the stored launch.  Per host thread, 4 entries, round-robin replacement.
+// ~100 cuTensorMapEncodeTiled calls and replays the stored launch.  Per host thread, 4 entries, round-robin replacement.  (TP_FUSE_ATTN,
+// TP_CHAIN and TP_GEMM_MODE only decide whether this plan runs at all, and are read before the cache is probed.)
 struct FwdKey {
   const void* packed; const void* x0; const void* xm; const void* layers[4]; void* out; void* ws; const void* peers[kMaxPeers];
   long long n, s0, sm, crop_rows;
-  int s, H, n_peers, sms, sch, noswz;
+  int s, H, n_peers, sms;
 };
 struct FwdPlan {
   FwdKey key;
@@ -1114,87 +1057,17 @@ int forward_impl(const void* packed, const void* x0, const void* xm, const void*
     for (int i = 0; i < n_peers && i < kMaxPeers; ++i) key.peers[i] = peer_out[i];
     key.n = n_crops; key.s0 = x0_crop_stride; key.sm = xm_crop_stride; key.crop_rows = out_crop_rows;
     key.s = s; key.H = H; key.n_peers = n_peers; key.sms = dev.sms;
-    {
-      const char* e1 = getenv("TP_SCHEDULE");
-      const char* e2 = getenv("TP_SEG_NOSWIZZLE");
-      key.sch = e1 != nullptr ? atoi(e1) : 0;
-      key.noswz = e2 != nullptr ? atoi(e2) : 0;
-    }
-    const bool feasible = chain_feasible(g, 8, dev.sms, false);
-    if (feasible) {
+    if (chain_feasible(g, 8, dev.sms, false)) {
       for (FwdPlan& fp : g_fwd_plans)
         if (fp.valid && memcmp(&fp.key, &key, sizeof(key)) == 0) {
           // (the counters were already reset by the memset above)
           TP_CUDA(launch_pdl(tp_gemm2_kernel, dim3(fp.launch.grid), dim3(kGemmThreads), Gemm2Config::kSmemBytes, stream, fp.launch.g, fp.launch.peers));
           return TP_OK;
         }
-    }
-    if (feasible) {
-      // Tile schedule (TP_SCHEDULE, read per call; default 0 = stage after stage).
-      //   1: [4] and [5] interleaved row block by row block ([5] five row blocks behind): the GELU epilogue of [4] (longer than its
-      //      K=1024 MMAs) then overlaps the K=4096 MMAs of [5] on every CTA pair instead of stalling the tensor pipe for a whole stage.
-      //   3: see below (wavefront over the last three stages only; for the fused all-gather).
-      //   4, 6: the batch as 2 / 4 sub-batches, each through all stages in turn (for the fused all-gather).
-      //   2: full software wavefront over groups of row blocks ([1] for group j, [2]k/v for j-1, KV-attention for j-2, [4] for j-3,
-      //      [5] for j-4).  An experiment, not the default: with every stage in flight the 73 MB of weights alone exceed the
-      //      50 MB L2, so the intermediates it means to keep on chip are evicted anyway.
-      const char* sch_env = getenv("TP_SCHEDULE");
-      const int sch = sch_env != nullptr ? atoi(sch_env) : 0;
-      SegPlan plan;
-      const long long nbR = (R + 255) / 256, nbQ = (Q + 255) / 256;
-      if (sch == 1) {
-        bool ok = true;
-        for (int i = 0; i < 6 && ok; ++i) ok = plan.add(i, 0, i == 3 || i == 4 ? nbQ : nbR, i == 3 || i == 4 ? nbQ : nbR);
-        const long long lag = 5;
-        for (long long j = 0; j < nbQ + lag && ok; ++j) ok = plan.add(6, j, j + 1, nbQ) && plan.add(7, j - lag, j - lag + 1, nbQ);
-        if (!ok) plan.n = 0;
-      } else if (sch == 3) {
-        // stages [1] [2] [3]q in order, then a wavefront over blocks of 256 queries: KV-attention tiles of block j, [4] of block j-1,
-        // [5] of block j-2.  Meant for the fused all-gather: [5]'s peer stores start flowing during the attention stage instead of
-        // all at the end, so the NVLink transfer (7/8 of the packed output per rank) hides under compute.
-        const int Wn = s * s;
-        long long GR = Wn;
-        while ((nbR + GR - 1) / GR > 100) GR *= 2;
-        const long long GQ = GR / Wn, NG = (nbR + GR - 1) / GR;
-        bool ok = true;
-        for (int i = 0; i < 5 && ok; ++i) ok = plan.add(i, 0, i == 3 || i == 4 ? nbQ : nbR, i == 3 || i == 4 ? nbQ : nbR);
-        for (long long j = 0; j <= NG + 2 && ok; ++j)
-          ok = plan.add(5, j * GR, (j + 1) * GR, nbR) && plan.add(6, (j - 1) * GQ, j * GQ, nbQ) && plan.add(7, (j - 2) * GQ, (j - 1) * GQ, nbQ);
-        if (!ok) plan.n = 0;
-      } else if (sch >= 4) {
-        // sub-batches: the batch is cut into (sch - 2) groups of query blocks; ALL stages of group g run (stage after stage) before
-        // group g+1 starts.  For the fused all-gather: the peer stores of group g's [5] tiles travel over NVLink while group g+1
-        // computes, so only the last group's share of the exchange is exposed.  The [1] / [2] ranges of a group reach 3 row blocks
-        // past its KV-attention range (a crop that straddles the group boundary needs its keys from both sides).
-        const int Wn = s * s;
-        const long long nsub = sch - 2;
-        const long long GQ = (nbQ + nsub - 1) / nsub > 0 ? (nbQ + nsub - 1) / nsub : 1, GR = GQ * Wn, NG = (nbQ + GQ - 1) / GQ;
-        bool ok = true;
-        for (long long gidx = 0; gidx < NG && ok; ++gidx) {
-          const bool last = gidx == NG - 1;
-          const long long r_lo = gidx == 0 ? 0 : gidx * GR + 3, r_hi = last ? nbR : (gidx + 1) * GR + 3;
-          const long long q_lo = gidx * GQ, q_hi = last ? nbQ : (gidx + 1) * GQ;
-          ok = plan.add(0, r_lo, r_hi, nbR) && plan.add(1, r_lo, r_hi, nbR) && plan.add(2, r_lo, r_hi, nbR) && plan.add(3, q_lo, q_hi, nbQ) &&
-               plan.add(4, q_lo, q_hi, nbQ) && plan.add(5, gidx * GR, last ? nbR : (gidx + 1) * GR, nbR) && plan.add(6, q_lo, q_hi, nbQ) &&
-               plan.add(7, q_lo, q_hi, nbQ);
-        }
-        if (!ok) plan.n = 0;
-      } else if (sch == 2) {
-        const int Wn = s * s;
-        long long GR = Wn > 8 ? Wn : 8;
-        while ((nbR + GR - 1) / GR > 48) GR *= 2;
-        const long long GQ = GR / Wn, NG = (nbR + GR - 1) / GR;
-        bool ok = plan.add(0, 0, GR, nbR) && plan.add(3, 0, nbQ, nbQ) && plan.add(4, 0, nbQ, nbQ);
-        for (long long j = 1; j <= NG + 4 && ok; ++j)
-          ok = plan.add(0, j * GR, (j + 1) * GR, nbR) && plan.add(1, (j - 1) * GR, j * GR, nbR) && plan.add(2, (j - 1) * GR, j * GR, nbR) &&
-               plan.add(5, (j - 2) * GR, (j - 1) * GR, nbR) && plan.add(6, (j - 3) * GQ, (j - 2) * GQ, nbQ) &&
-               plan.add(7, (j - 4) * GQ, (j - 3) * GQ, nbQ);
-        if (!ok) plan.n = 0;
-      }
       FwdPlan& slot = g_fwd_plans[g_fwd_next];
       g_fwd_next = (g_fwd_next + 1) % 4;
       slot.valid = false;
-      TP_TRY(launch_chain(g, 8, flags, W.n_flags, &front, dev.sms, stream, &plan, &slot.launch));
+      TP_TRY(launch_chain(g, 8, flags, W.n_flags, &front, dev.sms, stream, &slot.launch));
       slot.key = key;
       slot.valid = true;
       return TP_OK;
@@ -1411,21 +1284,6 @@ int tp_forward_host(const void* packed, const void* x0_host, const void* xm_host
   TP_CUDA(e3);
   return TP_OK;
 }
-
-#ifdef TP_GEMM_PROFILE
-// Profile builds only (libtokenpacker_b200_prof.so, not part of the public ABI): same as tp_gemm_bf16 plus a device
-// buffer [grid][16] of cycle counters of the pair kernel: {producer wait-empty, producer total, -, -, -, epilogue warp 0: MMA
-// k-loops (ring waits included), epilogue busy, -, accumulator transposes, slab hand-offs, slab-buffer waits}.
-TP_API int tp_gemm_bf16_prof(const void* a, int64_t lda, const void* b, int64_t ldb, void* c, int64_t ldc, int64_t m, int64_t n, int64_t k,
-                             const float* bias, int gelu, float alpha, long long* prof, void* stream) {
-  DeviceInfo dev;
-  TP_TRY(device_info(&dev));
-  GemmEpilogue ep = plain_epilogue(c, ldc, bias, gelu);
-  ep.alpha = alpha;
-  ep.prof = prof;
-  return launch_gemm(AOperand{a, lda, 0, 0}, b, ldb, m, n, k, ep, dev.sms, static_cast<cudaStream_t>(stream));
-}
-#endif
 
 int tp_gemm_tn_bf16(const void* a, int64_t lda, const void* b, int64_t ldb, void* c, int64_t ldc, int64_t m, int64_t n, int64_t k,
                     float alpha, void* stream) {

@@ -67,20 +67,7 @@ struct GemmEpilogue {
   int dual;                // 1 (with gelu): the bf16-rounded PRE-activation (after bias / LN fold, before GELU and alpha) is stored too,
                            // through GemmProblem::tmap_cx[0] (the training forward keeps z for GELU'(z); builder.py:66-75 under autograd).
                            // Pair kernel, plain (unsegmented) TMA-store output, two 64-column staging buffers per half.
-  long long* prof;         // TP_GEMM_PROFILE builds only: [grid][16] cycle counters (nullptr otherwise)
 };
-
-#ifndef TP_EPI_SUB_PAIRS
-#define TP_EPI_SUB_PAIRS 8      // column pairs per warp-uniform epilogue block: more independent chains for the scheduler, more registers
-#endif
-
-#ifdef TP_GEMM_PROFILE
-#define TP_PROF_T0() const long long prof_t0__ = clock64()
-#define TP_PROF_ADD(var) (var) += clock64() - prof_t0__
-#else
-#define TP_PROF_T0() do {} while (0)
-#define TP_PROF_ADD(var) do {} while (0)
-#endif
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;     // 64 bf16 = 128 bytes = one swizzle-128B row
@@ -215,22 +202,13 @@ struct PeerStores {
 };
 
 struct OutStage {
-  uint8_t* buf;              // this half's n_bufs x 16 KiB staging buffers (nullptr: direct 16-byte global stores)
-  uint64_t* full_bar;        // [n_bufs] slab written (count 4: one arrive per epilogue warp of the half) -> store warp
-  uint64_t* empty_bar;       // [n_bufs] slab's TMA store has finished reading the buffer (count 1, store warp) -> epilogue warps
-  int n_bufs;                // 2: slabs alternate buffers; 1: single buffer
-  uint32_t slab_seq;         // running slab number of this half (buffer = seq % n_bufs, mbarrier phase = seq / n_bufs)
-  bool swizzle;              // slab rows in the TMA swizzle of the row width (false: plain rows, for C maps built without swizzle)
+  uint8_t* buf;              // this half's 2 x 16 KiB staging buffers (nullptr: direct 16-byte global stores)
+  uint64_t* full_bar;        // [2] slab written (count 4: one arrive per epilogue warp of the half) -> store warp
+  uint64_t* empty_bar;       // [2] slab's TMA store has finished reading the buffer (count 1, store warp) -> epilogue warps
+  uint32_t slab_seq;         // running slab number of this half (buffer = seq % 2, mbarrier phase = seq / 2)
 };
-// Output slab = 128 rows x kSlabCols columns of bf16, in the TMA swizzle of that row width (64 columns: 128-byte rows,
-// SWIZZLE_128B; 32 columns: 64-byte rows, SWIZZLE_64B).  The narrow form halves the staging memory (32 KiB freed): not enough
-// for a fourth 48 KiB ring stage of the pair kernel, so it only matters with -DTP_OUT_BUFS=1 -DTP_SLAB_COLS=32 -DTP_PAIR_STAGES=4
-// (which gives up the dual pre-activation output of the training forward).
-#ifndef TP_SLAB_COLS
-#define TP_SLAB_COLS 64
-#endif
-constexpr int kSlabCols = TP_SLAB_COLS;
-static_assert(kSlabCols == 64 || kSlabCols == 32, "slab width: 64 (128B swizzle) or 32 (64B swizzle) columns");
+// Output slab = 128 rows x 64 columns of bf16: 128-byte rows in TMA's SWIZZLE_128B layout.
+constexpr int kSlabCols = 64;
 constexpr int kSlabRowBytes = kSlabCols * 2;
 constexpr int kChunksPerSlab = kSlabCols / 32;
 constexpr int kOutSlabBytes = 128 * kSlabRowBytes;
@@ -265,7 +243,7 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
 template <int kTileN>
 __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int N, const float (&acc)[2][kTileN / 4], uint32_t scratch,
                                               int row, int col_tile0, int quarter, int half, const float* s_col, const OutStage& out,
-                                              [[maybe_unused]] long long* pc = nullptr, long long c_extra = 0) {
+                                              long long c_extra = 0) {
   constexpr int kColsPerWarp = kTileN / 2;
   constexpr int kChunks = kColsPerWarp / 32;
   const bool ln_fold = ep.col_a != nullptr;
@@ -296,28 +274,22 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
   uint32_t r[32];
 #pragma unroll
   for (int chunk = 0; chunk < kChunks; ++chunk) {
-    {
-      TP_PROF_T0();
-      acc_chunk(acc, chunk, scratch, r);
-      TP_PROF_ADD(pc[0]);
-    }
+    acc_chunk(acc, chunk, scratch, r);
     const int col0 = col_tile0 + half * kColsPerWarp + chunk * 32;
     // dual output: every 64-column slab exists twice — pre-activation (even slab number, buffer 0) and activation (odd, buffer 1)
     const bool dual = ep.dual != 0 && out.buf != nullptr;
     const uint32_t slab_pre = out.slab_seq + 2u * static_cast<uint32_t>(chunk / kChunksPerSlab);
     const uint32_t slab_q = dual ? slab_pre + 1u : out.slab_seq + static_cast<uint32_t>(chunk / kChunksPerSlab);
-    const uint32_t slab_buf = slab_q & static_cast<uint32_t>(out.n_bufs - 1);
+    const uint32_t slab_buf = slab_q & 1u;
     if (out.buf != nullptr && (chunk % kChunksPerSlab) == 0) {
       // the TMA store that last used this staging buffer must have finished READING it (signalled by the store warp)
-      TP_PROF_T0();
       if (dual) mbar_wait(&out.empty_bar[slab_pre & 1u], ((slab_pre >> 1) & 1u) ^ 1u);
-      mbar_wait(&out.empty_bar[slab_buf], ((slab_q >> (out.n_bufs - 1)) & 1u) ^ 1u);
-      TP_PROF_ADD(pc[2]);
+      mbar_wait(&out.empty_bar[slab_buf], ((slab_q >> 1) & 1u) ^ 1u);
     }
     if (col0 < N) {        // N is a multiple of 32 (checked on the host) -> whole chunk in or out
       // kSubPairs packed pairs (2 columns each) go through every step together: each run-time option is ONE warp-uniform branch
-      // around a basic block of kSubPairs independent dependency chains for the scheduler to interleave.
-      constexpr int kSubPairs = TP_EPI_SUB_PAIRS;
+      // around a basic block of kSubPairs independent dependency chains for the scheduler to interleave (more chains, more registers).
+      constexpr int kSubPairs = 8;
       const int rloc = epi_row(quarter, lane_id());
 #pragma unroll
       for (int sub = 0; sub < 16 / kSubPairs; ++sub) {
@@ -345,7 +317,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
         }
         if (dual) {        // the pre-activation slab (same swizzled position in the other staging buffer)
           const uint32_t row_pre = out_addr + static_cast<uint32_t>((slab_pre & 1u) * kOutSlabBytes + rloc * kSlabRowBytes);
-          const int swz_pre = !out.swizzle ? 0 : (kSlabCols == 64 ? (rloc & 7) : ((rloc >> 1) & 3));
+          const int swz_pre = rloc & 7;
 #pragma unroll
           for (int g = 0; g < kSubPairs / 4; ++g) {
             uint32_t w[4];
@@ -384,10 +356,10 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
           }
         }
         if (out.buf != nullptr) {
-          // 16-byte piece index inside the slab row, XOR-swizzled like TMA does: 128-byte rows (SWIZZLE_128B) with (row & 7),
-          // 64-byte rows (SWIZZLE_64B) with ((row >> 1) & 3) — address bits [7,9/10) folded into bits [4,6/7)
+          // 16-byte piece index inside the slab row, XOR-swizzled like TMA's SWIZZLE_128B does for 128-byte rows: with (row & 7),
+          // address bits [7,10) folded into bits [4,7)
           const uint32_t row_base = out_addr + static_cast<uint32_t>(slab_buf * kOutSlabBytes + rloc * kSlabRowBytes);
-          const int swz = !out.swizzle ? 0 : (kSlabCols == 64 ? (rloc & 7) : ((rloc >> 1) & 3));
+          const int swz = rloc & 7;
 #pragma unroll
           for (int g = 0; g < kSubPairs / 4; ++g) {
             const int ci = (chunk % kChunksPerSlab) * 4 + sub * (kSubPairs / 4) + g;
@@ -426,14 +398,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
     }
     if (out.buf != nullptr && (chunk % kChunksPerSlab) == kChunksPerSlab - 1) {
       // slab complete: make the generic-proxy writes visible to the async proxy, then one arrive per warp hands it to the store warp
-      TP_PROF_T0();
       fence_proxy_async_smem();
       __syncwarp();
       if (lane_id() == 0) {
         if (dual) mbar_arrive(&out.full_bar[slab_pre & 1u]);
         mbar_arrive(&out.full_bar[slab_buf]);
       }
-      TP_PROF_ADD(pc[1]);
     }
   }
 }
@@ -671,7 +641,7 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       stage_col_vectors<kBlockN>(ep, N, n_blk * kBlockN, s_col, epi_tid, true);
       mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, half * kN * kBlockK * 2, full_bar, empty_bar, kStages, stage, phase,
                          num_k_blocks);
-      const OutStage no_stage{nullptr, nullptr, nullptr, 1, 0u, true};
+      const OutStage no_stage{nullptr, nullptr, nullptr, 0u};
       epilogue_tile<kBlockN>(ep, M, N, acc, scratch, m_blk * kBlockM + epi_row(quarter, lane), n_blk * kBlockN, quarter, half, s_col,
                              no_stage);
     }
@@ -687,14 +657,8 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 struct Gemm2Config {
   static constexpr int kTileM = 256;
   static constexpr int kTileN = 256;
-#ifndef TP_PAIR_STAGES
-#define TP_PAIR_STAGES 3
-#endif
-#ifndef TP_OUT_BUFS
-#define TP_OUT_BUFS 2
-#endif
-  static constexpr int kStages = TP_PAIR_STAGES;
-  static constexpr int kOutBufs = TP_OUT_BUFS;                   // staging buffers per column half (1 or 2)
+  static constexpr int kStages = 3;
+  static constexpr int kOutBufs = 2;                             // staging buffers per column half: consecutive slabs alternate
   static constexpr int kABytes = kBlockM * kBlockK * 2;          // this CTA's 128 rows of A
   static constexpr int kBBytes = kTileN * kBlockK * 2;           // the whole B tile
   static constexpr int kStageBytes = kABytes + kBBytes;          // 48 KiB
@@ -718,7 +682,6 @@ struct GemmProblem {
   CUtensorMap tmap_a2, tmap_b2;              // kind 1: the value operands (tmap_a / tmap_b: the key operands)
   int kind;              // 0: GEMM with the fused epilogue; 1: KV-attention tile (see attn_epilogue_tile)
   int c_wm_s;            // != 0: tmap_c is the 5-D window-major map of GemmEpilogue::wm_s
-  int c_noswz;           // 1: tmap_c (and the peer maps) were built WITHOUT swizzle: the epilogue writes plain slab rows
   AttnParams attn;
   CUtensorMap tmap_a_more[kMaxAParts - 1];   // A given as several tensors side by side along K (e.g. the four CLIP hidden states
                                              // that the reference concatenates, clip_encoder.py:28-44): part p covers k-blocks
@@ -771,27 +734,11 @@ struct FrontWork {
   int* done_counter;
 };
 
-// Optional tile schedule of a chained launch: instead of "stage after stage", the tile numbers run through SEGMENTS (problem,
-// first row block, number of row blocks) in the order the host lists them.  The fused forward interleaves the stages by groups of
-// row blocks with a fixed lag between producer and consumer stages (a software wavefront): intermediates are consumed while they
-// are still in L2, and epilogue-heavy tiles (GELU, attention) alternate with K=4096 tiles on every CTA pair, so neither the
-// tensor pipe nor the epilogue warps idle through a whole stage.  Any order in which every tile's producers have lower tile
-// numbers is deadlock-free.
-struct TileSeg {
-  int prob;       // index into GemmGroup::p
-  int m_lo;       // first 256-row block
-  int tile0;      // first tile number of the segment
-  int n_tiles;    // row blocks x n-blocks of the problem
-};
-constexpr int kMaxSegs = 384;
-
 struct GemmGroup {
   GemmProblem p[kMaxGroup];
   int count;
-  int total_tiles;
+  int total_tiles;            // tiles are numbered problem after problem
   FrontWork front;
-  int n_segs;                 // 0: tiles are numbered problem after problem
-  TileSeg segs[kMaxSegs];
 };
 
 struct TileRef {
@@ -801,22 +748,7 @@ struct TileRef {
   int split;
 };
 
-__device__ __forceinline__ TileRef decode_tile(const GemmGroup& g, int tile, int& cursor) {
-  if (g.n_segs != 0) {
-    // scheduled launch: every role walks its tiles in increasing order, so the segment cursor only moves forward
-    while (tile >= g.segs[cursor].tile0 + g.segs[cursor].n_tiles) ++cursor;
-    const TileSeg& sg = g.segs[cursor];
-    TileRef t;
-    t.pr = &g.p[sg.prob];
-    const int local = tile - sg.tile0;
-    const int mm = local / t.pr->num_n_blocks;
-    t.m_blk = sg.m_lo + mm;
-    t.n_blk = local - mm * t.pr->num_n_blocks;
-    t.split = 0;
-    t.kb0 = 0;
-    t.kb1 = t.pr->num_k_blocks;
-    return t;
-  }
+__device__ __forceinline__ TileRef decode_tile(const GemmGroup& g, int tile) {
   int p = 0;
   while (p + 1 < g.count && tile >= g.p[p].num_tiles) {
     tile -= g.p[p].num_tiles;
@@ -895,12 +827,10 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
     const int epi_tid = e * 32 + static_cast<int>(lane);
     const uint32_t scratch = smem_u32(s_scratch + e * kScratchBytesPerWarp);
     const int b_off = half * kN * kBlockK * 2;                  // this warpgroup's columns of the stage's B tile
-    int cursor = 0, stage = 0;
+    int stage = 0;
     uint32_t phase = 0;
     uint32_t slab_seq = 0;
     float acc[2][kN / 2];
-    [[maybe_unused]] long long w_acc = 0, t_work = 0;
-    [[maybe_unused]] long long pc[3] = {0, 0, 0};
     if (grp.front.x0 != nullptr) {
       // point queries: this CTA's share of the (query, 8-channel vector) items, 128 vectors per query
       const FrontWork& fw = grp.front;
@@ -937,7 +867,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       }
     }
     for (int tile = pair_idx; tile < num_tiles; tile += num_pairs) {
-      const TileRef t = decode_tile(grp, tile, cursor);
+      const TileRef t = decode_tile(grp, tile);
       const GemmProblem& pr = *t.pr;
       float* s_col = s_col_base;
       const int row_tile0 = t.m_blk * Cfg::kTileM + static_cast<int>(cta_rank) * kBlockM;
@@ -966,45 +896,28 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
         continue;
       }
       stage_col_vectors<kTileN>(pr.ep, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
-      {
-        TP_PROF_T0();
-        const int n_kb = t.kb1 - t.kb0;
-        if (pr.ab_mn_major == 1)
-          mma_tile<kN, 1, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
-        else if (pr.ab_mn_major == 2)
-          mma_tile<kN, 0, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
-        else
-          mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
-        TP_PROF_ADD(w_acc);
-      }
-      TP_PROF_T0();
+      const int n_kb = t.kb1 - t.kb0;
+      if (pr.ab_mn_major == 1)
+        mma_tile<kN, 1, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
+      else if (pr.ab_mn_major == 2)
+        mma_tile<kN, 0, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
+      else
+        mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
       const OutStage out{pr.use_tma_store ? s_out + half * Cfg::kOutBufs * kOutSlabBytes : nullptr, slab_full_bar + half * Cfg::kOutBufs,
-                         slab_empty_bar + half * Cfg::kOutBufs, Cfg::kOutBufs, slab_seq, pr.c_noswz == 0};
+                         slab_empty_bar + half * Cfg::kOutBufs, slab_seq};
       if (pr.use_tma_store) slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);     // slabs per tile and column half
-      epilogue_tile<kTileN>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, quarter, half, s_col, out, pc,
+      epilogue_tile<kTileN>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, quarter, half, s_col, out,
                             static_cast<long long>(t.split) * pr.c_split_stride);
-      TP_PROF_ADD(t_work);
     }
-#ifdef TP_GEMM_PROFILE
-    if (grp.p[0].ep.prof != nullptr && e == 0 && lane == 0) {
-      grp.p[0].ep.prof[blockIdx.x * 16 + 5] = w_acc;
-      grp.p[0].ep.prof[blockIdx.x * 16 + 6] = t_work;
-      grp.p[0].ep.prof[blockIdx.x * 16 + 8] = pc[0];          // epilogue warp 0: cycles in the accumulator transpose
-      grp.p[0].ep.prof[blockIdx.x * 16 + 9] = pc[1];         // ... in fence.proxy.async
-      grp.p[0].ep.prof[blockIdx.x * 16 + 10] = pc[2];          // ... in wait_group.read + named barrier
-    }
-#endif
   } else {
     setmaxnreg_dec<kAuxRegs>();
   if (warp_idx == kTmaWarp) {
     // ======================================= TMA producer (both CTAs) ============================
     // Whole warp runs the loop (uniform control flow); one elected lane issues the arrive + TMA instructions.
-    int stage = 0, cursor = 0;
+    int stage = 0;
     uint32_t phase = 0;
-    [[maybe_unused]] long long w_empty = 0;
-    [[maybe_unused]] const long long t_begin = clock64();
     for (int tile = pair_idx; tile < num_tiles; tile += num_pairs) {
-      const TileRef t = decode_tile(grp, tile, cursor);
+      const TileRef t = decode_tile(grp, tile);
       const GemmProblem& pr = *t.pr;
       const int row0 = t.m_blk * Cfg::kTileM + static_cast<int>(cta_rank) * kBlockM;          // my 128 rows of A
       const int brow0 = t.n_blk * kTileN;                                                     // the whole B tile
@@ -1066,11 +979,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
         srow1 = row0 + 64 - seg1 * pr.a_seg_rows;
       }
       for (int kb = t.kb0; kb < t.kb1; ++kb) {
-        {
-          TP_PROF_T0();
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          TP_PROF_ADD(w_empty);
-        }
+        mbar_wait(&empty_bar[stage], phase ^ 1u);
         if (elect_one()) {
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           uint8_t* sb = sa + Cfg::kABytes;
@@ -1103,12 +1012,6 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
     }
-#ifdef TP_GEMM_PROFILE
-    if (grp.p[0].ep.prof != nullptr && lane == 0) {
-      grp.p[0].ep.prof[blockIdx.x * 16 + 0] = w_empty;
-      grp.p[0].ep.prof[blockIdx.x * 16 + 1] = clock64() - t_begin;
-    }
-#endif
   } else if (warp_idx == kStoreWarp0 || warp_idx == kStoreWarp0 + 1) {
     // ======================================= store warps (both CTAs, one per column half) =========
     // Walks the same tile sequence as the epilogue warps of its half.  Per slab: wait until the 4 epilogue warps have written
@@ -1119,9 +1022,8 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
     uint64_t* full = slab_full_bar + half * Cfg::kOutBufs;
     uint64_t* empty = slab_empty_bar + half * Cfg::kOutBufs;
     uint32_t q = 0;
-    int cursor = 0;
     for (int tile = pair_idx; tile < num_tiles; tile += num_pairs) {
-      const TileRef t = decode_tile(grp, tile, cursor);
+      const TileRef t = decode_tile(grp, tile);
       const GemmProblem& pr = *t.pr;
       if (!pr.use_tma_store) continue;
       const int row_tile0 = t.m_blk * Cfg::kTileM + static_cast<int>(cta_rank) * kBlockM;
@@ -1129,8 +1031,8 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       const int n_maps = to_peers ? peers.count : 1;
       const int dual = pr.ep.dual != 0 ? 1 : 0;     // every column slab twice: pre-activation (tmap_cx[0]) then activation (tmap_c)
       for (int slab = 0; slab < (kTileN / 2 / kSlabCols) << dual; ++slab, ++q) {
-        const uint32_t buf = q & static_cast<uint32_t>(Cfg::kOutBufs - 1);
-        mbar_wait(&full[buf], (q >> (Cfg::kOutBufs - 1)) & 1u);
+        const uint32_t buf = q & 1u;
+        mbar_wait(&full[buf], (q >> 1) & 1u);
         {
           // Every TMA store of this slab is a JOB; lane l issues jobs l, l + 32, ...  All lanes walk the same (cheap) enumeration of the
           // slab's pieces and keep the parameters of their own jobs, then issue them together: the up to ~64 stores of a packed-row

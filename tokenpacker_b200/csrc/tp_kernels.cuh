@@ -446,14 +446,8 @@ __device__ __forceinline__ float hd_canvas_value(const HdImage& im, const float*
 // channel) pairs, and the lanes of a warp read neighbouring source pixels (a warp's load touches 4-6 sectors; with 4 pixels per
 // thread it was 16 sectors of which 6.5 bytes each were used, and the kernel sat at 18 % of DRAM waiting for L1).  Scalar stores of
 // 32 consecutive floats per warp.  The tap arithmetic is unchanged, so the bits are.
-#ifndef TP_HD_ROWS
-#define TP_HD_ROWS 8
-#endif
-#ifndef TP_HD_UNROLL
-#define TP_HD_UNROLL 2
-#endif
-constexpr int kHdRows = TP_HD_ROWS;                            // rows per thread; 336 = 42 x 8
-constexpr int kHdUnroll = TP_HD_UNROLL;                        // rows in flight per thread (loads of the next row issue under the math of this one)
+constexpr int kHdRows = 8;                                     // rows per thread; 336 = 42 x 8
+constexpr int kHdUnroll = 2;                                   // rows in flight per thread (loads of the next row issue under the math of this one)
 static_assert(kBlockPx % kHdRows == 0, "rows per CTA must divide the crop height");
 // Src: HdF32Source (tp_hd_tile_batch) or HdU8Source (tp_hd_preprocess_batch); Out: float or __nv_bfloat16.
 template <class Src, class Out>
