@@ -92,7 +92,9 @@ TP_API int tp_forward(const void* packed, const void* x0, const void* xm, int64_
  * (row stride H).  llava_arch.py:139-155 follows every crop's tokens with exactly one separator row (',' between columns, '\n'
  * at the end of a grid row and after the thumbnail), so the packed sequence of any batch of images is this layout with
  * out_crop_rows = M + 1 and the separator rows (tp_hd_fill_separators) in the gaps.  Unlike the seg_row_offset form the output
- * stays on the TMA-store path: each 128-row slab leaves as one clipped 3-D box per crop it touches.  out_crop_rows = 0 or M: dense. */
+ * stays on the TMA-store path: each 128-row slab leaves as one clipped 3-D box per crop it touches.  out_crop_rows = 0 or M: dense.
+ * Scale factors 8 and 24 (M = 9, 1: crops that are not a multiple of 4 rows) have no such boxes: their rows are stored one by one
+ * by the one-CTA GEMM kernels, whatever the batch size or TP_GEMM_MODE. */
 TP_API int tp_forward_packed(const void* packed, const void* x0, const void* xm, int64_t n_crops, int64_t x0_crop_stride,
                              int64_t xm_crop_stride, int scale_factor, int hidden, void* out, int64_t out_crop_rows,
                              void* workspace, size_t workspace_bytes, void* stream);
@@ -112,7 +114,9 @@ TP_API int tp_forward_layers(const void* packed, const void* const* layers, int6
  * produces them — no separate collective kernel, no staging copy and, with R = M + 1, no assembly pass either: the stores land
  * in the packed per-image sequences of llava_arch.py:139-155 directly (separator rows: tp_hd_fill_separators on each rank).
  * The caller must run a cross-rank barrier after the stream reaches this call before any rank reads its buffer.
- * Needs hidden % 256 == 0.  Replaces: encode_images on sharded crops + the cross-rank reassembly of llava_arch.py:139-155. */
+ * Needs hidden % 256 == 0.  The packed form (out_crop_rows > M) needs M to be a multiple of 4 rows: at scale factors 8 and 24 it
+ * returns TP_ERR_INVALID_ARGUMENT before launching anything (their dense form works).
+ * Replaces: encode_images on sharded crops + the cross-rank reassembly of llava_arch.py:139-155. */
 TP_API int tp_forward_allgather(const void* packed, const void* x0, const void* xm, int64_t n_crops, int64_t x0_crop_stride,
                                 int64_t xm_crop_stride, int scale_factor, int hidden, void* const* peer_out, int n_peers,
                                 int64_t crop_offset, int64_t out_crop_rows, void* workspace, size_t workspace_bytes, void* stream);

@@ -113,6 +113,15 @@ int make_map_wm(CUtensorMap* map, const void* ptr, long long rows, long long col
   return encode_bf16_map(map, ptr, 5, dims, strides, box);
 }
 
+// Height of the smallest store box of a uniform-stride segmented output (packed HD rows): gcd(seg_len, 128).  Every piece of a
+// 128-row slab that belongs to one segment is a multiple of it.  The pair kernel's segmented stores need it to be at least 4, which
+// rules out scale factors 8 and 24 (M = 9, 1); the one-CTA kernels store such rows one by one.
+int seg_store_unit(long long seg_len) {
+  int unit = 128;
+  while (seg_len % unit != 0) unit >>= 1;
+  return unit;
+}
+
 struct DeviceInfo {
   int sms;
 };
@@ -312,9 +321,8 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
     } else if (c_segmented) {
       if (it.ep.seg_len <= 0 || it.M % it.ep.seg_len != 0 || it.ep.seg_stride < it.ep.seg_len) return TP_ERR_INVALID_ARGUMENT;
       p.c_seg_len = it.ep.seg_len;
-      p.c_unit = 128;
-      while (it.ep.seg_len % p.c_unit != 0) p.c_unit >>= 1;          // gcd(seg_len, 128)
-      if (p.c_unit < 4) return TP_ERR_INVALID_ARGUMENT;             // (scale factors with < 4 tokens per crop keep the row-offset path)
+      p.c_unit = seg_store_unit(it.ep.seg_len);
+      if (p.c_unit < 4) return TP_ERR_INVALID_ARGUMENT;             // (choose_kernel sends these to the one-CTA kernels' row stores)
       for (int lvl = 0; lvl < kBoxLevels; ++lvl) {
         int rows = p.c_unit << lvl;
         if (rows > kBlockM || rows > it.ep.seg_len) rows = p.c_unit;  // level never used (pieces are at most min(seg_len, 128) rows)
@@ -451,7 +459,10 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
 // =3 pair kernel without grouping (A/B experiments; read per call, no caching).
 // Returns 0 pair, 1 one-CTA 256, 2 one-CTA 128, or -1 (invalid).
 int choose_kernel(const GemmItem& it, int count, int sms, int mode) {
-  const bool pair_ok = (it.N % 256 == 0) && sms >= 2;
+  // a uniform-stride segmented output whose crops are not a multiple of 4 rows cannot leave through the pair kernel's boxes
+  // (launch_gemm_pair_group rejects it): cost-based, forced and chained selection all fall back to the one-CTA kernels then
+  const bool c_segmented = it.ep.seg_row_offset == nullptr && !it.ep.out_f32 && it.ep.seg_stride != 0 && it.ep.seg_stride != it.ep.seg_len;
+  const bool pair_ok = (it.N % 256 == 0) && sms >= 2 && !(c_segmented && seg_store_unit(it.ep.seg_len) < 4);
   const bool pair_only = it.n_peers > 0 || it.tn || it.ep.dual || it.a.parts > 1 || it.k_splits > 1 || it.ep.out_f32 || it.kind == 1 || it.ep.wm_s != 0;   // pair-kernel-only features
   if (pair_only && !pair_ok) return -1;
   const bool needs_256 = it.ep.stats_out != nullptr;                        // statistics slots assume 256-column tiles
@@ -1173,6 +1184,9 @@ int tp_forward_allgather(const void* packed, const void* x0, const void* xm, int
   if (scale_factor <= 0 || kGrid % scale_factor != 0) return TP_ERR_BAD_SCALE_FACTOR;
   const int g = kGrid / scale_factor;
   if (out_crop_rows != 0 && out_crop_rows < g * g) return TP_ERR_INVALID_ARGUMENT;
+  // packed rows reach the peers only through the pair kernel's segmented stores: rejected here, before anything is launched, for the
+  // scale factors those stores cannot serve (8 and 24)
+  if (out_crop_rows != 0 && out_crop_rows != g * g && seg_store_unit(g * g) < 4) return TP_ERR_INVALID_ARGUMENT;
   const size_t crop_rows = out_crop_rows != 0 ? static_cast<size_t>(out_crop_rows) : static_cast<size_t>(g) * g;
   const size_t slot = static_cast<size_t>(crop_offset) * crop_rows * hidden * 2;   // this rank's first row in every peer's output buffer
   void* dst[kMaxPeers];

@@ -1035,7 +1035,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
         mbar_wait(&full[buf], (q >> 1) & 1u);
         {
           // Every TMA store of this slab is a JOB; lane l issues jobs l, l + 32, ...  All lanes walk the same (cheap) enumeration of the
-          // slab's pieces and keep the parameters of their own jobs, then issue them together: the up to ~64 stores of a packed-row
+          // slab's pieces and keep the parameters of their own jobs, then issue them together: the up to 88 stores of a packed-row
           // slab that goes to eight GPUs leave the warp in two or three instructions instead of one lane issuing them one by one.
           const uint8_t* src = s_out + (half * Cfg::kOutBufs + static_cast<int>(buf)) * kOutSlabBytes;
           const int col = t.n_blk * kTileN + half * (kTileN / 2) + (slab >> dual) * kSlabCols;

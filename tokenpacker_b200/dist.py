@@ -77,7 +77,9 @@ class FusedGatherTokenPacker:
     remaining tiles' math.  ``forward_hd`` goes one step further: the stores land in the PACKED per-image rows of
     llava_arch.py:139-155 on every rank (uniform crop stride M + 1, see ``tp_forward_packed``), so there is no gathered
     intermediate and no assembly pass — each rank only fills the separator rows of its own copy.  CUDA + NCCL-capable ranks of
-    one NVLink domain only; inference only.
+    one NVLink domain only; inference only.  ``forward_hd`` needs crops of a multiple of 4 tokens: scale factors 8 and 24 (9 and 1
+    tokens) raise TokenPackerError (invalid argument) from tp_forward_allgather, which launches no projector work for them;
+    ``forward_gathered`` serves them.
 
     Two buffers alternate between calls, so ONE cross-rank barrier per call is enough: the barrier of call i+1 (which
     every rank reaches only after its stream has consumed call i's buffer) is what licenses call i+2 to overwrite that buffer."""
