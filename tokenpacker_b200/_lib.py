@@ -1,7 +1,8 @@
 """ctypes binding of libtokenpacker_b200.so — the thin seam between the Python host code and the C-ABI CUDA library.
 
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
-Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h and include/tokenpacker_b200_input_grad.h one to one.
+Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h and
+include/tokenpacker_b200_input_grad.h one to one.
 """
 from __future__ import annotations
 
@@ -51,6 +52,18 @@ class TpHdU8Source(C.Structure):
     """tp_hd_u8_source (include/tokenpacker_b200_hd_u8.h): where one decoded 8-bit image lies (element strides of channel, row
     and column)."""
     _fields_ = [("pixels", C.c_void_p), ("stride_c", C.c_int64), ("stride_y", C.c_int64), ("stride_x", C.c_int64)]
+
+
+class TpClipImage(C.Structure):
+    """tp_clip_image (include/tokenpacker_b200_clip_u8.h): one row of the non-HD CLIP preprocessing plan."""
+    _fields_ = [(n, C.c_int32) for n in ("h", "w", "canvas_h", "canvas_w", "pad_y", "pad_x", "resized_h", "resized_w", "top", "left",
+                                         "ksize_x", "ksize_y")] + \
+               [("coeff_x", C.c_int64), ("coeff_y", C.c_int64), ("row0", C.c_int32), ("rows", C.c_int32),
+                ("workspace_offset", C.c_int64), ("workspace_row", C.c_int64)]
+
+
+TP_CLIP_SQUARE = 0
+TP_CLIP_PAD = 1
 
 
 # name -> (restype, argtypes); kept as data so tests can check the header and the binding agree
@@ -107,6 +120,14 @@ HD_U8_SIGNATURES = {
     "tp_hd_preprocess_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
 }
 
+# the same for include/tokenpacker_b200_clip_u8.h (decoded 8-bit images into the non-HD CLIP input: pad / square)
+CLIP_U8_SIGNATURES = {
+    "tp_clip_preprocess_plan": (C.c_int, [C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.c_int64, C.c_int, C.POINTER(TpClipImage),
+                                          C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_size_t)]),
+    "tp_clip_preprocess_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_size_t, C.c_void_p]),
+}
+
 # the same for include/tokenpacker_b200_input_grad.h (gradients w.r.t. the CLIP features in the training path)
 INPUT_GRAD_SIGNATURES = {
     "tp_backward_inputs": (C.c_int, [C.POINTER(TpWeights), C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p,
@@ -120,7 +141,7 @@ def _load():
             f"tokenpacker_b200: {LIB_PATH} is missing. Build it with `make -C tokenpacker_b200/csrc` "
             "(or `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES}.items():
+    for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

@@ -7,8 +7,12 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <map>
+#include <tuple>
+#include <vector>
 
 #include "../../include/tokenpacker_b200.h"
+#include "../../include/tokenpacker_b200_clip_u8.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"
 #include "tp_gemm.cuh"
@@ -1509,6 +1513,171 @@ int tp_hd_preprocess_batch(const tp_hd_image* images_dev, const tp_hd_u8_source*
   else
     hd_tile_batch_kernel<<<static_cast<unsigned>(blocks), kBlockPx, 0, stream>>>(images, crop_table_dev, n_crops, src,
                                                                                 static_cast<__nv_bfloat16*>(crops));
+  TP_CUDA(cudaGetLastError()); ++g_launch_count;
+  return TP_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Non-HD CLIP input: expand2square + PIL 8-bit BICUBIC resize + center crop (include/tokenpacker_b200_clip_u8.h)
+// ------------------------------------------------------------------------------------------------
+namespace {
+// The coefficient arithmetic below restates Pillow's Resample.c (bicubic_filter, precompute_coeffs, normalize_coeffs_8bpc) operation
+// for operation in double precision; PIL's bits depend on every product being rounded before the following addition.  A compiler
+// that contracts a * b + c into one fused multiply-add (g++ does by default on aarch64, where FMA is part of the base ISA) would
+// round once instead of twice and move some weights by one unit, so contraction is switched off for these functions.
+__attribute__((optimize("fp-contract=off"))) double pil_bicubic(double x) {
+  const double a = -0.5;
+  if (x < 0.0) x = -x;
+  if (x < 1.0) return ((a + 2.0) * x - (a + 3.0)) * x * x + 1;
+  if (x < 2.0) return (((x - 5) * x + 8) * x - 4) * a;
+  return 0.0;
+}
+
+int pil_bicubic_ksize(int in_size, int out_size) {
+  const double scale = static_cast<double>(in_size) / out_size;
+  return static_cast<int>(ceil(2.0 * (scale < 1.0 ? 1.0 : scale))) * 2 + 1;
+}
+
+// Weights of the outputs first .. first + 336 - 1 of an in_size -> out_size BICUBIC resample, laid out as tp_clip_image documents:
+// [336] first source index, [336] tap count, [ksize][336] int32 weights (zero past the count).  tab may be NULL (bounds only).
+__attribute__((optimize("fp-contract=off"))) void pil_bicubic_table(int in_size, int out_size, int first, int32_t* tab, int* lo, int* hi) {
+  const double scale = static_cast<double>(in_size) / out_size;
+  const double filterscale = scale < 1.0 ? 1.0 : scale;
+  const double support = 2.0 * filterscale;
+  const double ss = 1.0 / filterscale;
+  const int ksize = pil_bicubic_ksize(in_size, out_size);
+  std::vector<double> w(ksize);
+  *lo = INT_MAX; *hi = 0;
+  for (int j = 0; j < kBlockPx; ++j) {
+    const int xx = first + j;
+    const double center = (xx + 0.5) * scale;
+    int xmin = static_cast<int>(center - support + 0.5);
+    if (xmin < 0) xmin = 0;
+    int xmax = static_cast<int>(center + support + 0.5);
+    if (xmax > in_size) xmax = in_size;
+    xmax -= xmin;
+    if (xmin < *lo) *lo = xmin;
+    if (xmin + xmax > *hi) *hi = xmin + xmax;
+    if (tab == nullptr) continue;
+    double ww = 0.0;
+    for (int x = 0; x < xmax; ++x) {
+      w[x] = pil_bicubic((x + xmin - center + 0.5) * ss);
+      ww += w[x];
+    }
+    tab[j] = xmin;
+    tab[kBlockPx + j] = xmax;
+    for (int x = 0; x < ksize; ++x) {
+      int32_t k = 0;
+      if (x < xmax) {
+        const double v = ww != 0.0 ? w[x] / ww : w[x];
+        k = static_cast<int32_t>(v < 0 ? -0.5 + v * (1 << kClipPrecision) : 0.5 + v * (1 << kClipPrecision));
+      }
+      tab[(2 + x) * kBlockPx + j] = k;
+    }
+  }
+}
+}  // namespace
+
+int tp_clip_preprocess_plan(const int64_t* h, const int64_t* w, int64_t n_images, int mode, tp_clip_image* images, int32_t* coeffs,
+                            int64_t* n_coeffs, size_t* workspace_bytes) {
+  static_assert(sizeof(tp_clip_image) == sizeof(ClipImage), "tp_clip_image and the kernel's ClipImage must have the same layout");
+  if (h == nullptr || w == nullptr || n_coeffs == nullptr || workspace_bytes == nullptr || n_images < 0 ||
+      (mode != TP_CLIP_SQUARE && mode != TP_CLIP_PAD))
+    return TP_ERR_INVALID_ARGUMENT;
+  for (int64_t b = 0; b < n_images; ++b)
+    if (h[b] < 1 || w[b] < 1 || h[b] > TP_CLIP_MAX_SIDE || w[b] > TP_CLIP_MAX_SIDE) return TP_ERR_INVALID_ARGUMENT;
+  const bool write = images != nullptr && coeffs != nullptr;
+  struct Table { int in, out, first; int64_t offset; int lo, hi; };
+  std::map<std::tuple<int, int, int>, Table> tables;         // one table per (input size, output size, first kept output)
+  int64_t n_co = 0, ws_rows = 0;
+  auto table = [&](int in, int out, int first) -> const Table& {
+    auto it = tables.find(std::make_tuple(in, out, first));
+    if (it == tables.end()) {
+      Table t{in, out, first, n_co, 0, 0};
+      pil_bicubic_table(in, out, first, write ? coeffs + n_co : nullptr, &t.lo, &t.hi);
+      n_co += static_cast<int64_t>(2 + pil_bicubic_ksize(in, out)) * kBlockPx;
+      it = tables.emplace(std::make_tuple(in, out, first), t).first;
+    }
+    return it->second;
+  };
+  for (int64_t b = 0; b < n_images; ++b) {
+    tp_clip_image im;
+    memset(&im, 0, sizeof(im));
+    im.h = static_cast<int32_t>(h[b]); im.w = static_cast<int32_t>(w[b]);
+    im.canvas_h = im.h; im.canvas_w = im.w;
+    if (mode == TP_CLIP_PAD && im.h != im.w) {               // expand2square (mm_utils.py:14-25): paste into the middle of L x L
+      const int side = im.h > im.w ? im.h : im.w;
+      im.canvas_h = im.canvas_w = side;
+      if (im.w > im.h) im.pad_y = (im.w - im.h) / 2; else im.pad_x = (im.h - im.w) / 2;
+    }
+    // get_resize_output_image_size(default_to_square=False): the short edge becomes 336, the long edge int(336 * long / short)
+    // (Python's true division, float64, truncated); nothing is resized when the short edge is already 336
+    const bool w_short = im.canvas_w <= im.canvas_h;
+    const int s = w_short ? im.canvas_w : im.canvas_h, l = w_short ? im.canvas_h : im.canvas_w;
+    im.resized_h = im.canvas_h; im.resized_w = im.canvas_w;
+    if (s != kBlockPx) {
+      const int new_l = static_cast<int>(static_cast<double>(static_cast<int64_t>(kBlockPx) * l) / static_cast<double>(s));
+      im.resized_h = w_short ? new_l : kBlockPx;
+      im.resized_w = w_short ? kBlockPx : new_l;
+    }
+    im.top = (im.resized_h - kBlockPx) / 2;
+    im.left = (im.resized_w - kBlockPx) / 2;
+    im.coeff_x = im.coeff_y = -1;
+    if (im.resized_w != im.canvas_w) {
+      const Table& t = table(im.canvas_w, im.resized_w, im.left);
+      im.ksize_x = pil_bicubic_ksize(t.in, t.out);
+      im.coeff_x = t.offset;
+    }
+    im.row0 = im.top;
+    im.rows = kBlockPx;
+    if (im.resized_h != im.canvas_h) {
+      const Table& t = table(im.canvas_h, im.resized_h, im.top);
+      im.ksize_y = pil_bicubic_ksize(t.in, t.out);
+      im.coeff_y = t.offset;
+      im.row0 = t.lo;
+      im.rows = t.hi - t.lo;
+    }
+    if (im.ksize_x == 0) im.rows = 0;                         // no horizontal pass: the vertical pass reads the canvas
+    im.workspace_row = ws_rows;
+    im.workspace_offset = ws_rows * kClipRowBytes;
+    ws_rows += im.rows;
+    if (write) images[b] = im;
+  }
+  *n_coeffs = n_co;
+  *workspace_bytes = static_cast<size_t>(ws_rows) * kClipRowBytes;
+  return TP_OK;
+}
+
+int tp_clip_preprocess_batch(const tp_clip_image* images_host, const tp_clip_image* images_dev, const tp_hd_u8_source* sources_dev,
+                             const int32_t* coeffs_dev, int64_t n_images, const float* norm_table_dev, int out_dtype, void* out,
+                             void* workspace, size_t workspace_bytes, void* stream_) {
+  if (images_host == nullptr || images_dev == nullptr || sources_dev == nullptr || coeffs_dev == nullptr || norm_table_dev == nullptr ||
+      out == nullptr || n_images < 0 || (out_dtype != 0 && out_dtype != 1))
+    return TP_ERR_INVALID_ARGUMENT;
+  if (n_images == 0) return TP_OK;
+  if (n_images > 0x7fffffffll / kBlockPx) return TP_ERR_INVALID_ARGUMENT;      // the vertical launch: one CTA per output row
+  int64_t rows = 0;
+  for (int64_t b = 0; b < n_images; ++b) {
+    const tp_clip_image& im = images_host[b];
+    if (im.rows < 0 || im.workspace_row < 0) return TP_ERR_INVALID_ARGUMENT;
+    if (im.ksize_x > 0 && im.workspace_row + im.rows > rows) rows = im.workspace_row + im.rows;
+  }
+  if (rows > 0x7fffffffll) return TP_ERR_INVALID_ARGUMENT;                       // the horizontal launch: one CTA per workspace row
+  if (static_cast<uint64_t>(rows) * kClipRowBytes > workspace_bytes) return TP_ERR_WORKSPACE_TOO_SMALL;
+  if (rows > 0 && workspace == nullptr) return TP_ERR_INVALID_ARGUMENT;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const ClipImage* images = reinterpret_cast<const ClipImage*>(images_dev);
+  const HdU8Image* sources = reinterpret_cast<const HdU8Image*>(sources_dev);
+  unsigned char* ws = static_cast<unsigned char*>(workspace);
+  if (rows > 0) {
+    clip_resample_h_kernel<<<static_cast<unsigned>(rows), kBlockPx, 0, stream>>>(images, n_images, sources, coeffs_dev, ws);
+    TP_CUDA(cudaGetLastError()); ++g_launch_count;
+  }
+  const unsigned blocks = static_cast<unsigned>(n_images * kBlockPx);
+  if (out_dtype == 0)
+    clip_resample_v_kernel<<<blocks, kBlockPx, 0, stream>>>(images, sources, coeffs_dev, ws, norm_table_dev, static_cast<float*>(out));
+  else
+    clip_resample_v_kernel<<<blocks, kBlockPx, 0, stream>>>(images, sources, coeffs_dev, ws, norm_table_dev, static_cast<__nv_bfloat16*>(out));
   TP_CUDA(cudaGetLastError()); ++g_launch_count;
   return TP_OK;
 }

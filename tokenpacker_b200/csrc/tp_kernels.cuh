@@ -510,6 +510,115 @@ __global__ void __launch_bounds__(kBlockPx) hd_tile_batch_kernel(const HdImage* 
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Non-HD CLIP input (tp_clip_preprocess_batch): expand2square onto a virtual canvas (pad mode), PIL's 8-bit BICUBIC resize of the
+// short edge to 336, center crop, and the (channel, byte) table.  PIL's fixed-point arithmetic exactly: int32 weights with 22 fraction
+// bits from the host plan, an accumulator that starts at 1 << 21, clamp(acc >> 22, 0, 255); the horizontal pass first, rounded to
+// uint8 in the workspace, then the vertical pass.  Every sum is an exact integer sum (255 * sum |k| < 2^31), so its order is free.
+// Only the 336 kept columns and the canvas rows the kept output rows read are computed.
+// ------------------------------------------------------------------------------------------------
+struct ClipImage {          // mirrors tp_clip_image (include/tokenpacker_b200_clip_u8.h)
+  int h, w, canvas_h, canvas_w, pad_y, pad_x, resized_h, resized_w, top, left, ksize_x, ksize_y;
+  long long coeff_x, coeff_y;
+  int row0, rows;
+  long long workspace_offset, workspace_row;
+};
+
+constexpr int kClipPrecision = 22;
+constexpr int kClipRowBytes = kBlockPx * 3;                   // one workspace row: 336 kept columns x 3 channels, uint8
+
+__device__ __forceinline__ int clip_u8(int acc) { return min(max(acc >> kClipPrecision, 0), 255); }   // Resample.c clip8
+
+// Pixel (y, x, ch) of the canvas: the source inside the pasted rectangle, expand2square's background (122, 116, 104), the CLIP mean
+// as int(x * 255), outside it.  In square mode the canvas is the source and every read is inside.
+struct ClipCanvas {
+  const unsigned char* p;
+  long long sc, sy, sx;
+  int h, w, py, px;
+  __device__ __forceinline__ ClipCanvas(const ClipImage& im, const HdU8Image& s)
+      : p(s.pixels), sc(s.stride_c), sy(s.stride_y), sx(s.stride_x), h(im.h), w(im.w), py(im.pad_y), px(im.pad_x) {}
+  __device__ __forceinline__ int at(int y, int x, int ch) const {
+    const int yy = y - py, xx = x - px;
+    if (static_cast<unsigned>(yy) < static_cast<unsigned>(h) && static_cast<unsigned>(xx) < static_cast<unsigned>(w))
+      return __ldg(p + yy * sy + xx * sx + ch * sc);
+    return ch == 0 ? 122 : (ch == 1 ? 116 : 104);
+  }
+};
+
+// Horizontal pass.  CTA = one workspace row (one canvas row of one image), thread = one kept output column, 3 channels.  The image is
+// the last one whose first workspace row is <= this row (images skipping this pass own no rows).  Weight table: tap-major
+// [ksize][336], so the lanes of a warp read consecutive weights.
+__global__ void __launch_bounds__(kBlockPx) clip_resample_h_kernel(const ClipImage* __restrict__ images, long long n_images,
+                                                                   const HdU8Image* __restrict__ sources, const int* __restrict__ coeffs,
+                                                                   unsigned char* __restrict__ workspace) {
+  const long long row = blockIdx.x;
+  long long lo = 0, hi = n_images - 1;
+  while (lo < hi) {                                              // uniform over the CTA
+    const long long mid = (lo + hi + 1) / 2;
+    if (images[mid].workspace_row <= row) lo = mid; else hi = mid - 1;
+  }
+  const ClipImage im = images[lo];
+  const int r = static_cast<int>(row - im.workspace_row);
+  if (im.ksize_x == 0 || r >= im.rows) return;                   // only past the last image's rows (an oversized workspace)
+  const ClipCanvas cv(im, sources[lo]);
+  const int y = im.row0 + r, x = threadIdx.x;
+  const int* tab = coeffs + im.coeff_x;
+  const int xmin = __ldg(tab + x), n = __ldg(tab + kBlockPx + x);
+  const int* k = tab + 2 * kBlockPx + x;
+  int a0 = 1 << (kClipPrecision - 1), a1 = a0, a2 = a0;
+  for (int i = 0; i < n; ++i) {
+    const int kk = __ldg(k + i * kBlockPx);
+    a0 += kk * cv.at(y, xmin + i, 0);
+    a1 += kk * cv.at(y, xmin + i, 1);
+    a2 += kk * cv.at(y, xmin + i, 2);
+  }
+  unsigned char* o = workspace + im.workspace_offset + static_cast<long long>(r) * kClipRowBytes + x * 3;
+  o[0] = static_cast<unsigned char>(clip_u8(a0));
+  o[1] = static_cast<unsigned char>(clip_u8(a1));
+  o[2] = static_cast<unsigned char>(clip_u8(a2));
+}
+
+// Vertical pass, byte lookup and store.  CTA = one output row of one image, thread = one output column, 3 channels.  The row's taps
+// are the same for every thread (broadcast loads).  Its input is the workspace when the horizontal pass ran, else the canvas at the
+// crop's columns; when the vertical pass is skipped the output row is input row `top + y`, as PIL leaves it.
+template <class Out>
+__global__ void __launch_bounds__(kBlockPx) clip_resample_v_kernel(const ClipImage* __restrict__ images, const HdU8Image* __restrict__ sources,
+                                                                   const int* __restrict__ coeffs, const unsigned char* __restrict__ workspace,
+                                                                   const float* __restrict__ table, Out* __restrict__ out) {
+  __shared__ float lut[kNormTable];
+  for (int i = threadIdx.x; i < kNormTable; i += blockDim.x) lut[i] = __ldg(table + i);
+  __syncthreads();
+  const long long b = blockIdx.x / kBlockPx;
+  const int y = static_cast<int>(blockIdx.x % kBlockPx), x = threadIdx.x;
+  const ClipImage im = images[b];
+  const ClipCanvas cv(im, sources[b]);
+  const bool from_ws = im.ksize_x > 0;
+  const unsigned char* ws = workspace + (from_ws ? im.workspace_offset : 0) + x * 3;
+  auto in = [&](int canvas_row, int ch) -> int {                 // pixel (canvas_row, kept column x) after the horizontal pass
+    return from_ws ? __ldg(ws + static_cast<long long>(canvas_row - im.row0) * kClipRowBytes + ch) : cv.at(canvas_row, im.left + x, ch);
+  };
+  int v[3];
+  if (im.ksize_y > 0) {
+    const int* tab = coeffs + im.coeff_y;
+    const int ymin = __ldg(tab + y), n = __ldg(tab + kBlockPx + y);
+    const int* k = tab + 2 * kBlockPx + y;
+    int a0 = 1 << (kClipPrecision - 1), a1 = a0, a2 = a0;
+    for (int i = 0; i < n; ++i) {
+      const int kk = __ldg(k + i * kBlockPx);
+      a0 += kk * in(ymin + i, 0);
+      a1 += kk * in(ymin + i, 1);
+      a2 += kk * in(ymin + i, 2);
+    }
+    v[0] = clip_u8(a0); v[1] = clip_u8(a1); v[2] = clip_u8(a2);
+  } else {
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) v[ch] = in(im.top + y, ch);
+  }
+  Out* o = out + (b * 3 * kBlockPx + y) * kBlockPx + x;
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) hd_store(o + static_cast<long long>(ch) * kBlockPx * kBlockPx, lut[ch * 256 + v[ch]]);
+}
+
 // out[seg_row_offset[c] + m, :] = feats[c, m, :]  (bf16; one thread per 8 channels): crop token blocks -> packed rows.
 __global__ void scatter_crops_kernel(const __nv_bfloat16* __restrict__ feats, long long n_crops, int tokens, int hidden,
                                      const long long* __restrict__ seg_row_offset, __nv_bfloat16* __restrict__ out) {

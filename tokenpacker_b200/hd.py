@@ -191,14 +191,10 @@ def _norm_table_on(device) -> torch.Tensor:
     return t
 
 
-def hd_preprocess_batch(images, patch_num: int = 9, dtype=torch.float32, layout: str = "HWC", _return_launch: bool = False):
-    """ToTensor + Normalize (train.py:645) and the tiling block (train.py:695-731) for a batch of DECODED 8-bit images, in one launch.
-
-    images: sequence of uint8 CUDA tensors, [h, w, 3] for layout "HWC" (np.array(pil_image), what the reference decodes) or [3, h, w]
-    for "CHW" (torchvision.io.decode_image); sizes may differ, and views are read through their strides, not copied.
-    dtype: torch.float32, or torch.bfloat16 (the tower's dtype; equal to the float32 crops .to(torch.bfloat16), bit for bit).
-    Returns (crops [sum_i n_crops_i, 3, 336, 336] in dtype, h_block list, w_block list) in the reference's crop order.  The float32
-    crops have exactly the bits hd_tile_batch gives for the same images normalised on the host (norm_table)."""
+def _u8_sources(images, dtype, layout: str):
+    """Checks shared by the entry points that read decoded 8-bit images: the output dtype, the layout, and every image uint8, CUDA,
+    [h, w, 3] ("HWC") or [3, h, w] ("CHW"), on one device.  Returns (images as a list, device, (h, w) per image, and per image
+    (pixels, stride_c, stride_y, stride_x) of tp_hd_u8_source: views are read through their strides, not copied)."""
     if dtype not in (torch.float32, torch.bfloat16):
         raise ValueError(f"dtype must be torch.float32 or torch.bfloat16, not {dtype}")
     if layout not in ("HWC", "CHW"):
@@ -223,6 +219,18 @@ def hd_preprocess_batch(images, patch_num: int = 9, dtype=torch.float32, layout:
     else:
         sizes = [(int(im.shape[1]), int(im.shape[2])) for im in images]
         sources = [(im.data_ptr(), im.stride(0), im.stride(1), im.stride(2)) for im in images]
+    return images, device, sizes, sources
+
+
+def hd_preprocess_batch(images, patch_num: int = 9, dtype=torch.float32, layout: str = "HWC", _return_launch: bool = False):
+    """ToTensor + Normalize (train.py:645) and the tiling block (train.py:695-731) for a batch of DECODED 8-bit images, in one launch.
+
+    images: sequence of uint8 CUDA tensors, [h, w, 3] for layout "HWC" (np.array(pil_image), what the reference decodes) or [3, h, w]
+    for "CHW" (torchvision.io.decode_image); sizes may differ, and views are read through their strides, not copied.
+    dtype: torch.float32, or torch.bfloat16 (the tower's dtype; equal to the float32 crops .to(torch.bfloat16), bit for bit).
+    Returns (crops [sum_i n_crops_i, 3, 336, 336] in dtype, h_block list, w_block list) in the reference's crop order.  The float32
+    crops have exactly the bits hd_tile_batch gives for the same images normalised on the host (norm_table)."""
+    images, device, sizes, sources = _u8_sources(images, dtype, layout)
     table = _norm_table_on(device)
     out_dtype = 0 if dtype == torch.float32 else 1
 
