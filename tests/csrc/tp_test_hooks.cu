@@ -1,5 +1,6 @@
 // Test-only entry points into the backward's internal kernels and the forward's buffer layouts (libtokenpacker_b200_testhooks.so,
-// loaded by tests/test_train_kernels_gpu.py and tests/test_forward_stages_gpu.py; never by the package).  The library is the product translation unit plus the tpt_* functions
+// loaded by tests/test_train_kernels_gpu.py, tests/test_forward_stages_gpu.py and tests/test_train_stages_gpu.py; never by the
+// package).  The library is the product translation unit plus the tpt_* functions
 // below, which call the same launch functions tp_backward calls (tp_train.inl), so every kernel runs with the launch configuration
 // of a training step.  Conventions as in include/tokenpacker_b200.h: device pointers, caller-owned buffers, work enqueued on
 // ``stream``, a tp_status returned.
@@ -106,6 +107,36 @@ TP_API int tpt_work_layout(int64_t n_crops, int s, int hidden, int64_t* out) {
     out[2 * i + 1] = bytes[i];
   }
   out[24] = static_cast<int64_t>(L.total);
+  return TP_OK;
+}
+
+// Buffer layouts of the training step for (n_crops, s, hidden), so that a test reads every activation tp_forward_train saves and
+// every intermediate tp_backward forms where they were put: out[2 i], out[2 i + 1] = byte offset and byte size of region i, first
+// the 14 SavedLayout regions of ``saved`` (z_kv, h_kv, y_k, y_v, stats, k_p, v_p, q, y_q, q_p, ctx, o, z_m, h_m), then the 22
+// BwdLayout regions of the backward workspace (w_m2t, g_t, hm_t, dzm, d_o, dctx, dqp, dkp, dvp, lnq_t, lnk_t, lnv_t, dqh, dkh, dvh,
+// dyq, dyk, dyv, dzkv, ln_part, col_part, splitk); out[72] = the saved total, out[73] = the workspace total.  A region the
+// configuration does not allocate (the transposing fallback's scratch when hidden % 256 == 0) has size 0.  The sizes are the
+// regions' shapes (the layouts' comments); the gaps up to the next offset are alignment padding that nothing writes.
+TP_API int tpt_train_layout(int64_t n_crops, int s, int hidden, int64_t* out) {
+  if (out == nullptr || n_crops <= 0 || s <= 0 || kGrid % s != 0 || !valid_hidden(hidden)) return TP_ERR_INVALID_ARGUMENT;
+  const SavedLayout S = saved_layout(n_crops, s, hidden);
+  const BwdLayout B = bwd_layout(n_crops, s, hidden);
+  const long long R = n_crops * kTokens, Q = n_crops * (kGrid / s) * (kGrid / s), H = hidden;
+  const long long act = R * kC * 2, qry = Q * kC * 2, fb = (H % 256 != 0) ? H * B.Qp * 2 : 0;
+  const size_t off[36] = {S.z_kv, S.h_kv, S.y_k, S.y_v, S.stats, S.k_p, S.v_p, S.q, S.y_q, S.q_p, S.ctx, S.o, S.z_m, S.h_m,
+                          B.w_m2t, B.g_t, B.hm_t, B.dzm, B.d_o, B.dctx, B.dqp, B.dkp, B.dvp, B.lnq_t, B.lnk_t, B.lnv_t, B.dqh, B.dkh,
+                          B.dvh, B.dyq, B.dyk, B.dyv, B.dzkv, B.ln_part, B.col_part, B.splitk};
+  const long long bytes[36] = {2 * act, 2 * act, act, act, (2 * R + Q) * kStatSlots * 2 * 4, act, act, qry, qry, qry, qry, qry, Q * H * 2,
+                               Q * H * 2,
+                               (H % 256 != 0) ? H * H * 2 : 0, fb, fb, Q * H * 2, qry, qry, qry, act, act, qry, act, act, qry, act, act,
+                               qry, act, act, 2 * act, 3ll * kLnBlocks * 3 * kC * 4, static_cast<long long>(kColChunks) * (H > 2048 ? H : 2048) * 4,
+                               2ll * kWgradSplits * kC * kC * 4};
+  for (int i = 0; i < 36; ++i) {
+    out[2 * i] = static_cast<int64_t>(off[i]);
+    out[2 * i + 1] = bytes[i];
+  }
+  out[72] = static_cast<int64_t>(S.total);
+  out[73] = static_cast<int64_t>(B.total);
   return TP_OK;
 }
 

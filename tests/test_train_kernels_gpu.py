@@ -245,6 +245,36 @@ def _ln_ref(y, stats, gamma):
     return yh, rstd, rho, dyh
 
 
+def _ln_bwd_ref(gout, y, stats, gamma, ln_blocks):
+    """fp64 LayerNorm backward (ln_bwd_kernel + ln_param_reduce_kernel over ln_blocks CTAs) from the bf16 / fp32 values the kernels
+    read: {name: (ref, floor)} for dy, dgamma and dbeta, and the length of the fp32 chain of the column sums (dbias, taken over the
+    STORED dy, has the same chain).  Floors: 48 E per row sum (32 sequential lane adds + 5 shuffle levels), propagated through rstd
+    and yhat; column sums: rows-per-warp + 8 warps + 19 + 16 lane partials."""
+    rows = y.shape[0]
+    yh, rstd, rho, dyh = _ln_ref(y, stats, gamma)
+    g, gm = gout.to(F64), gamma.to(F64)
+    gg = gm * g
+    c1, c2 = gg.mean(-1), (gg * yh).mean(-1)
+    ref = rstd[:, None] * (gg - c1[:, None] - yh * c2[:, None])
+    A, B, Y = gg.abs().mean(-1), (gg * yh).abs().mean(-1), yh.abs().amax(-1)
+    dc1 = 48 * E * A
+    dc2 = 48 * E * B + A * dyh
+    mag = gg.abs().amax(-1) + c1.abs() + Y * c2.abs()
+    floor = rstd * (dc1 + Y * dc2 + c2.abs() * dyh) + (rho + 4 * E) * rstd * mag
+    warps = ln_blocks * 8
+    chain = (rows + warps - 1) // warps + 8 + (ln_blocks + 15) // 16 + 16 + 2
+    return {"dy": (ref, floor[:, None]),
+            "dgamma": ((g * yh).sum(0), chain * E * (g * yh).abs().sum(0) + (g.abs() * dyh[:, None]).sum(0)),
+            "dbeta": (g.sum(0), chain * E * g.abs().sum(0))}, chain
+
+
+def _ln_apply_ref(y, stats, gamma, beta):
+    """fp64 LayerNorm output yhat gamma + beta (ln_apply_kernel) and its floor: the fp32 error of yhat, then one fma"""
+    yh, _, _, dyh = _ln_ref(y, stats, gamma)
+    gm, bt = gamma.to(F64), beta.to(F64)
+    return yh * gm + bt, gm.abs() * dyh[:, None] + 2 * E * ((yh * gm).abs() + bt.abs())
+
+
 @pytest.mark.parametrize("rows", [1, 7, 296 * 8 + 3, 16704])
 def test_ln_bwd_and_param_reduce(hk, record_property, rows):
     """dy = rstd (gg - mean(gg) - yhat mean(gg yhat)) elementwise, dgamma / dbeta (column sums of g yhat / g) and dbias (column sums of
@@ -262,27 +292,13 @@ def test_ln_bwd_and_param_reduce(hk, record_property, rows):
     lnout = torch.empty(rows, 1024, dtype=BF, device="cuda")
     assert hk.tpt_ln_apply(P(y), P(stats), P(gamma), P(beta), P(lnout), rows) == 0
 
-    yh, rstd, rho, dyh = _ln_ref(y, stats, gamma)
-    g, gm, bt = gout.to(F64), gamma.to(F64), beta.to(F64)
-    gg = gm * g
-    c1, c2 = gg.mean(-1), (gg * yh).mean(-1)
-    ref = rstd[:, None] * (gg - c1[:, None] - yh * c2[:, None])
-    A, B, Y = gg.abs().mean(-1), (gg * yh).abs().mean(-1), yh.abs().amax(-1)
-    dc1 = 48 * E * A
-    dc2 = 48 * E * B + A * dyh
-    mag = gg.abs().amax(-1) + c1.abs() + Y * c2.abs()
-    floor = rstd * (dc1 + Y * dc2 + c2.abs() * dyh) + (rho + 4 * E) * rstd * mag
-    _check(record_property, "dy", dy, ref, floor[:, None])
-
-    warps = hk.ln_blocks * 8
-    chain = (rows + warps - 1) // warps + 8 + (hk.ln_blocks + 15) // 16 + 16 + 2
-    _check(record_property, "dgamma", dgam, (g * yh).sum(0), chain * E * (g * yh).abs().sum(0) + (g.abs() * dyh[:, None]).sum(0))
-    _check(record_property, "dbeta", dbet, g.sum(0), chain * E * g.abs().sum(0))
+    refs, chain = _ln_bwd_ref(gout, y, stats, gamma, hk.ln_blocks)
+    _check(record_property, "dy", dy, *refs["dy"])
+    _check(record_property, "dgamma", dgam, *refs["dgamma"])
+    _check(record_property, "dbeta", dbet, *refs["dbeta"])
     dyk = dy.to(F64)
     _check(record_property, "dbias", dbias, dyk.sum(0), chain * E * dyk.abs().sum(0))
-
-    ref_ln = yh * gm + bt
-    _check(record_property, "ln_apply", lnout, ref_ln, gm.abs() * dyh[:, None] + 2 * E * ((yh * gm).abs() + bt.abs()))
+    _check(record_property, "ln_apply", lnout, *_ln_apply_ref(y, stats, gamma, beta))
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -390,6 +406,13 @@ def _cdf(zd):
     return 0.5 * torch.special.erfc(-zd / math.sqrt(2))
 
 
+def _gelu_grad_ref(zd):
+    """fp64 GELU'(z) = Phi(z) + z phi(z) and the floor of gelu_grad's fp32 value: 1.5e-7 (erf) + a few E + |z phi| (__expf: 2^-21
+    + z^2 E relative) + 2^-126 (exp flushed to zero)"""
+    zphi = zd * _phi(zd)
+    return _cdf(zd) + zphi, 1.5e-7 + 8 * E + zphi.abs() * (2.0 ** -21 + zd * zd * E + 4 * E) + 2.0 ** -126
+
+
 def test_gelu_fwd_every_bf16(hk, record_property):
     """gelu_fwd_kernel against the fp64 erf GELU x Phi(x) at all 65280 finite bf16 inputs.  Floor: Abramowitz & Stegun 7.1.28
     (|erf error| <= 3e-7, so 1.5e-7 |x|) + a few fp32 roundings of |x|, + 2^-133 for results in bf16's subnormal range.
@@ -411,10 +434,7 @@ def test_gelu_grad_every_bf16(hk, record_property):
     part = torch.empty(hk.col_chunks * 256, dtype=torch.float32, device="cuda")
     out = torch.empty(256, dtype=BF, device="cuda")
     assert hk.tpt_gelu_bwd_bias(P(dz), P(z), 256, z.shape[0], 256, P(out), None, P(part), part.numel()) == 0
-    zd = z.to(F64)
-    zphi = zd * _phi(zd)
-    ref = _cdf(zd) + zphi
-    _check(record_property, "gelu_grad", dz, ref, 1.5e-7 + 8 * E + zphi.abs() * (2.0 ** -21 + zd * zd * E + 4 * E) + 2.0 ** -126)
+    _check(record_property, "gelu_grad", dz, *_gelu_grad_ref(z.to(F64)))
 
 
 @pytest.mark.parametrize("mode", ["1", "2"])
@@ -436,6 +456,12 @@ def test_gemm_gelu_epilogue_equals_gelu_kernel_bitwise(hk, monkeypatch, mode):
 # ------------------------------------------------------------------------------------------------------------------------------
 # column sums (bias gradients)
 # ------------------------------------------------------------------------------------------------------------------------------
+def _colsum_chain(rows, col_chunks):
+    """longest fp32 chain of colsum_partial + colsum_reduce over rows: rows per chunk + 16 lanes of chunks + the 16 lane sums + 2"""
+    chunks = min(rows, col_chunks)
+    return (rows + chunks - 1) // chunks + (chunks + 15) // 16 + 16 + 2
+
+
 @pytest.mark.parametrize("cols", [8, 1000, 2048, 5120])
 @pytest.mark.parametrize("rows", [1, 591, 592, 593, 36864])
 def test_colsum(hk, record_property, rows, cols):
@@ -444,7 +470,6 @@ def test_colsum(hk, record_property, rows, cols):
     stored, bit for bit.  Floor: one fp32 chain of rows-per-chunk + 37 + 16 adds.  Measured on an H100: worst error / bound 0.978."""
     ld = cols + 16 if rows == 593 else cols                    # a strided input
     x = _bf((rows, ld), rows * 7 + cols, mean=0.3)
-    chunks = min(rows, hk.col_chunks)
     part = torch.empty(hk.col_chunks * cols, dtype=torch.float32, device="cuda")
     scale = 0.08838834764831845 if cols == 1000 else 1.0
     outs = []
@@ -454,7 +479,7 @@ def test_colsum(hk, record_property, rows, cols):
         outs.append(out)
     assert torch.equal(outs[0].view(torch.int16), outs[1].view(torch.int16))
     xd = x[:, :cols].to(F64)
-    chain = (rows + chunks - 1) // chunks + (chunks + 15) // 16 + 16 + 2
+    chain = _colsum_chain(rows, hk.col_chunks)
     _check(record_property, "colsum", outs[0], scale * xd.sum(0), scale * chain * E * xd.abs().sum(0))
 
     z = _bf((rows, ld), rows + cols + 1, scale=2.0)
