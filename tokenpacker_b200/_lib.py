@@ -1,8 +1,8 @@
 """ctypes binding of libtokenpacker_b200.so — the thin seam between the Python host code and the C-ABI CUDA library.
 
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
-Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h and
-include/tokenpacker_b200_input_grad.h one to one.
+Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
+include/tokenpacker_b200_input_grad.h and include/tokenpacker_b200_layers.h one to one.
 """
 from __future__ import annotations
 
@@ -134,6 +134,17 @@ INPUT_GRAD_SIGNATURES = {
                                      C.c_void_p, C.POINTER(TpWeights), C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
+# the same for include/tokenpacker_b200_layers.h (training and packed HD output straight from the four CLIP hidden states)
+LAYERS_SIGNATURES = {
+    "tp_forward_train_layers": (C.c_int, [C.POINTER(TpWeights), C.c_void_p, C.POINTER(C.c_void_p), C.c_int64, C.c_int64, C.c_int, C.c_int,
+                                          C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "tp_backward_layers": (C.c_int, [C.POINTER(TpWeights), C.c_void_p, C.POINTER(C.c_void_p), C.c_int64, C.c_int64, C.c_int, C.c_int,
+                                     C.c_void_p, C.c_void_p, C.POINTER(TpWeights), C.POINTER(C.c_void_p), C.c_int64, C.c_void_p,
+                                     C.c_size_t, C.c_void_p]),
+    "tp_forward_layers_packed": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                           C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+}
+
 
 def _load():
     if not os.path.exists(LIB_PATH):
@@ -141,7 +152,8 @@ def _load():
             f"tokenpacker_b200: {LIB_PATH} is missing. Build it with `make -C tokenpacker_b200/csrc` "
             "(or `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES}.items():
+    for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
+                                      **LAYERS_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

@@ -15,6 +15,7 @@
 #include "../../include/tokenpacker_b200_clip_u8.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"
+#include "../../include/tokenpacker_b200_layers.h"
 #include "tp_gemm.cuh"
 #include "tp_kernels.cuh"
 #include "tp_backward.cuh"
@@ -181,6 +182,11 @@ struct GemmItem {
   int n_peers = 0;
   int tn = 0;                      // 1: C[M,N] = A^T . B with A given as [K, M] (ld = a.ld) and B as [K, N] (ld = ldb), both row-major
                                    // 2: C[M,N] = A . B with A the usual [M, K] and B given as [K, N] row-major (dgrad with the weight as stored)
+  // tn == 1 only: B as b_parts tensors side by side along N (b, then b_more; same ldb and segmentation), each [K, N / b_parts], and
+  // b_seg_rows != 0: B's K rows in segments of b_seg_rows rows, b_seg_stride elements apart (a [:,1:] view of CLIP hidden states)
+  const void* b_more[3] = {nullptr, nullptr, nullptr};
+  int b_parts = 1;
+  long long b_seg_rows = 0, b_seg_stride = 0;
   // kind 1 (KV-attention, pair kernel only): a / b = y_k (window-major rows) and the gamma-folded W_ik; a2 / b2 = y_v and W_iv;
   // M = rows of y_k, N = K = 1024; attn holds everything else; dep / dep2 / dep3 = the producers of y_k, y_v and q'
   int kind = 0;
@@ -210,6 +216,7 @@ int check_item(const GemmItem& it) {
     return TP_ERR_INVALID_ARGUMENT;
   if (it.ep.stats_out != nullptr && (it.N % 256 != 0 || it.ep.stats_out_slots != it.N / 128)) return TP_ERR_INVALID_ARGUMENT;
   if (it.ep.col_a != nullptr && (it.ep.stats_in == nullptr || it.ep.stats_in_slots <= 0)) return TP_ERR_INVALID_ARGUMENT;
+  if ((it.b_parts != 1 || it.b_seg_rows != 0) && it.tn != 1) return TP_ERR_INVALID_ARGUMENT;
   return TP_OK;
 }
 
@@ -283,7 +290,26 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
       total += p.num_tiles;
       continue;
     }
-    if (it.tn == 1) {
+    if (it.tn == 1 && (it.b_parts > 1 || it.b_seg_rows != 0)) {
+      // row-major [K, M] A as below; B split along N into parts of whole 256-column tiles, each a 2-D [K, N / parts] map or a 3-D
+      // (cols, row in segment, segment) map with the same 64 x 64 boxes
+      if (it.b_parts < 1 || it.b_parts > kMaxAParts || it.N % (it.b_parts * Cfg::kTileN) != 0 || it.a.parts > 1 || it.a.seg_rows != 0 ||
+          (it.b_seg_rows != 0 && (it.b_seg_rows % kBlockK != 0 || it.K % it.b_seg_rows != 0)))
+        return TP_ERR_INVALID_ARGUMENT;
+      TP_TRY(make_map_2d(&p.tmap_a, it.a.ptr, it.K, it.M, it.a.ld, 64));
+      const long long np = it.N / it.b_parts;
+      for (int q = 0; q < it.b_parts; ++q) {
+        const void* ptr = q == 0 ? it.b : it.b_more[q - 1];
+        CUtensorMap* map = q == 0 ? &p.tmap_b : &p.tmap_a_more[q - 1];
+        if (ptr == nullptr) return TP_ERR_INVALID_ARGUMENT;
+        if (it.b_seg_rows == 0) TP_TRY(make_map_2d(map, ptr, it.K, np, it.ldb, 64));
+        else TP_TRY(make_map_3d(map, ptr, it.K / it.b_seg_rows, it.b_seg_rows, np, it.ldb, it.b_seg_stride, 64));
+      }
+      p.b_parts = it.b_parts;
+      p.b_nblocks_per_part = static_cast<int>(np / Cfg::kTileN);
+      p.b_seg_rows = static_cast<int>(it.b_seg_rows);
+      p.ab_mn_major = 1;
+    } else if (it.tn == 1) {
       // row-major [K, M] / [K, N] operands: box = 64 MN-elements x 64 K-rows
       TP_TRY(make_map_2d(&p.tmap_a, it.a.ptr, it.K, it.M, it.a.ld, 64));
       TP_TRY(make_map_2d(&p.tmap_b, it.b, it.K, it.N, it.ldb, 64));
@@ -374,9 +400,13 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
   memset(&peers, 0, sizeof(peers));
   int peer_item = -1;
   // The destination maps of the launch: the peers of a fused all-gather, or — for a segmented (packed-row) output that stays on this
-  // GPU — the local buffer as the one "destination" (same store path, including the whole-segment boxes).
+  // GPU — the local buffer as the one "destination" (same store path, including the whole-segment boxes).  Further local segmented
+  // outputs whose segments exceed a slab (no whole-segment boxes: the input gradients of the four CLIP layers, 576-row crops) store
+  // through their own tmap_c / tmap_cx maps, which cut a slab into the same pieces; a slab of such an output is at most two pieces of
+  // at most 7 boxes each (unit >= 4), well inside the store warp's 96 job slots.
   for (int i = 0; i < count; ++i)
     if (items[i].n_peers > 0 || g.p[i].c_seg_len != 0) {
+      if (peer_item >= 0 && items[i].n_peers == 0 && items[peer_item].n_peers == 0 && g.p[i].c_seg_len > kBlockM) continue;
       if (peer_item >= 0) return TP_ERR_INVALID_ARGUMENT;      // one set of destination maps per launch
       peer_item = i;
     }
@@ -939,6 +969,15 @@ struct FwdPlan {
 thread_local FwdPlan g_fwd_plans[4];
 thread_local int g_fwd_next = 0;
 
+// Checks of the entry points in include/tokenpacker_b200_layers.h, before any CUDA call: every layer given and 16-byte aligned, crops
+// crop_stride elements apart (at least 576 rows of 1024, a 16-byte multiple: TMA strides)
+int check_layers(const void* const* layers, int64_t crop_stride) {
+  if (layers == nullptr || crop_stride < static_cast<int64_t>(kTokens) * kC || crop_stride % 8 != 0) return TP_ERR_INVALID_ARGUMENT;
+  for (int i = 0; i < 4; ++i)
+    if (layers[i] == nullptr || (reinterpret_cast<uintptr_t>(layers[i]) & 15) != 0) return TP_ERR_INVALID_ARGUMENT;
+  return TP_OK;
+}
+
 // xm_layers != nullptr: the multi-level stack is given as its four [n_crops, 576, 1024] layers (row stride 1024, crop stride
 // xm_crop_stride) instead of one [n_crops, 576, 4096] tensor; ``xm`` is then ignored.
 int forward_impl(const void* packed, const void* x0, const void* xm, const void* const* xm_layers, int64_t n_crops, int64_t x0_crop_stride,
@@ -1178,6 +1217,18 @@ int tp_forward_layers(const void* packed, const void* const* layers, int64_t n_c
                       void* out, const int64_t* seg_row_offset, void* workspace, size_t workspace_bytes, void* stream) {
   if (layers == nullptr) return TP_ERR_INVALID_ARGUMENT;
   return forward_impl(packed, layers[3], nullptr, layers, n_crops, crop_stride, crop_stride, scale_factor, hidden, out, seg_row_offset, 0,
+                      nullptr, 0, workspace, workspace_bytes, stream);
+}
+
+int tp_forward_layers_packed(const void* packed, const void* const* layers, int64_t n_crops, int64_t crop_stride, int scale_factor,
+                             int hidden, void* out, int64_t out_crop_rows, void* workspace, size_t workspace_bytes, void* stream) {
+  if (scale_factor <= 0 || kGrid % scale_factor != 0) return TP_ERR_BAD_SCALE_FACTOR;
+  TP_TRY(check_layers(layers, crop_stride));
+  const int64_t mq = static_cast<int64_t>(kGrid / scale_factor) * (kGrid / scale_factor);
+  if ((reinterpret_cast<uintptr_t>(out) & 15) != 0 || !valid_hidden(hidden) ||
+      (out_crop_rows != 0 && (out_crop_rows < mq || out_crop_rows > 0x7fffffffll / hidden)))
+    return TP_ERR_INVALID_ARGUMENT;
+  return forward_impl(packed, layers[3], nullptr, layers, n_crops, crop_stride, crop_stride, scale_factor, hidden, out, nullptr, out_crop_rows,
                       nullptr, 0, workspace, workspace_bytes, stream);
 }
 

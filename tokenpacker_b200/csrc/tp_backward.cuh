@@ -524,19 +524,13 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
 // backward; 0.25 x is exact in fp32, so the bits match given the same dq.  Writes every element, zeros included.
 // One thread per 8 channels of one fine token.
 // ------------------------------------------------------------------------------------------------
+// The 8 bf16 values of fine token t of crop n, channels [8 vec, 8 vec + 8)
 template <int S>
-__global__ void __launch_bounds__(256) point_query_bwd_kernel(const __nv_bfloat16* __restrict__ dq, __nv_bfloat16* __restrict__ dx0,
-                                                              long long n_tokens) {
+__device__ __forceinline__ uint4 point_query_bwd_value(const __nv_bfloat16* __restrict__ dq, long long n, int t, int vec) {
   constexpr int G = kGrid / S;
   constexpr int M = G * G;
   constexpr int kLo = (S % 2 == 1) ? (S - 1) / 2 : S / 2 - 1;     // first tap row / column inside the window
   constexpr int kHi = (S % 2 == 1) ? kLo : kLo + 1;               // last
-  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  const long long tok = idx >> 7;            // 128 vectors of 8 channels per token
-  const int vec = static_cast<int>(idx & 127);
-  if (tok >= n_tokens) return;
-  const long long n = tok / kTokens;
-  const int t = static_cast<int>(tok - n * kTokens);
   const int r = t / kGrid, c = t - r * kGrid;
   const int hb = r / S, wb = c / S;
   const int ri = r - hb * S, ci = c - wb * S;
@@ -553,7 +547,41 @@ __global__ void __launch_bounds__(256) point_query_bwd_kernel(const __nv_bfloat1
       out = pack8(f);
     }
   }
-  *reinterpret_cast<uint4*>(dx0 + tok * kC + vec * 8) = out;
+  return out;
+}
+
+template <int S>
+__global__ void __launch_bounds__(256) point_query_bwd_kernel(const __nv_bfloat16* __restrict__ dq, __nv_bfloat16* __restrict__ dx0,
+                                                              long long n_tokens) {
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long tok = idx >> 7;            // 128 vectors of 8 channels per token
+  const int vec = static_cast<int>(idx & 127);
+  if (tok >= n_tokens) return;
+  const long long n = tok / kTokens;
+  const int t = static_cast<int>(tok - n * kTokens);
+  *reinterpret_cast<uint4*>(dx0 + tok * kC + vec * 8) = point_query_bwd_value<S>(dq, n, t, vec);
+}
+
+// The same stencil ADDED to a crop-strided destination that already holds another gradient of the same tensor (CLIP layer 23 is both
+// feat and the last quarter of feat_multi): dx = bf16(float(dx) + float(v)) with v the bf16 value point_query_bwd_kernel stores —
+// autograd's bf16 sum of the two paths.  Every token is read, modified and written, so a -0.0 left by the other path becomes
+// -0.0 + +0.0 = +0.0 on the tokens the stencil does not touch, exactly as the sum makes it.
+template <int S>
+__global__ void __launch_bounds__(256) point_query_bwd_acc_kernel(const __nv_bfloat16* __restrict__ dq, __nv_bfloat16* __restrict__ dx,
+                                                                  long long crop_stride, long long n_tokens) {
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long tok = idx >> 7;
+  const int vec = static_cast<int>(idx & 127);
+  if (tok >= n_tokens) return;
+  const long long n = tok / kTokens;
+  const int t = static_cast<int>(tok - n * kTokens);
+  uint4* p = reinterpret_cast<uint4*>(dx + n * crop_stride + static_cast<long long>(t) * kC + vec * 8);
+  float a[8], b[8];
+  unpack8(*p, a);
+  unpack8(point_query_bwd_value<S>(dq, n, t, vec), b);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) a[i] = __fadd_rn(a[i], b[i]);
+  *p = pack8(a);
 }
 
 }  // namespace tp

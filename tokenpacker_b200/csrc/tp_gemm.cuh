@@ -688,6 +688,11 @@ struct GemmProblem {
                                              // [p * a_kblocks_per_part, (p+1) * a_kblocks_per_part)
   int a_parts;           // 1: a single A tensor
   int a_kblocks_per_part;
+  // TN form (ab_mn_major == 1) only, where A is never split: B given as several tensors side by side along N (the four CLIP hidden
+  // states as the wgrad operand of k/v_proj.0), part p > 0 in tmap_a_more[p - 1]; part = n-block / b_nblocks_per_part
+  int b_parts;           // 0 or 1: a single B tensor
+  int b_nblocks_per_part;
+  int b_seg_rows;        // TN form: 0: plain 2-D B; else rows per segment of the 3-D (cols, row, segment) B map (a multiple of 64)
   int M, N, K;
   int a_seg_rows;        // 0: plain 2-D A; else rows per segment of the 3-D (crop-strided) A map
   int ab_mn_major;       // 1: BOTH operands are given as row-major [K, M] / [K, N] matrices (wgrad: C = A^T . B, contraction over rows)
@@ -740,6 +745,9 @@ struct GemmGroup {
   int total_tiles;            // tiles are numbered problem after problem
   FrontWork front;
 };
+
+// __grid_constant__ parameters of tp_gemm2_kernel: the kernel parameter space of sm_90 holds 32764 bytes
+static_assert(sizeof(GemmGroup) + sizeof(PeerStores) <= 32764, "tp_gemm2_kernel's parameter block exceeds the 32 KB limit");
 
 struct TileRef {
   const GemmProblem* pr;
@@ -1002,10 +1010,28 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
           if (pr.ab_mn_major == 0) {
             tma_load_2d(sb, &pr.tmap_b, &full_bar[stage], kb * kBlockK, brow0);
             tma_load_2d(sb + Cfg::kBBytes / 2, &pr.tmap_b, &full_bar[stage], kb * kBlockK, brow0 + kTileN / 2);
-          } else {                                       // 1 (TN) and 2 (NN): B is a row-major [K, N] matrix
+          } else if (pr.b_parts <= 1 && pr.b_seg_rows == 0) {   // 1 (TN) and 2 (NN): B is a row-major [K, N] matrix
 #pragma unroll
             for (int a4 = 0; a4 < 4; ++a4)
               tma_load_2d(sb + a4 * (Cfg::kBBytes / 4), &pr.tmap_b, &full_bar[stage], brow0 + a4 * 64, kb * kBlockK);
+          } else {
+            // TN form with B split along N: the part that holds this tile's 256 columns, and the tile's first column inside it
+            const int bpart = pr.b_parts > 1 ? t.n_blk / pr.b_nblocks_per_part : 0;
+            const CUtensorMap* tb = bpart == 0 ? &pr.tmap_b : &pr.tmap_a_more[bpart - 1];
+            const int bcol0 = bpart == 0 ? brow0 : (t.n_blk - bpart * pr.b_nblocks_per_part) * kTileN;
+            if (pr.b_seg_rows == 0) {
+#pragma unroll
+              for (int a4 = 0; a4 < 4; ++a4)
+                tma_load_2d(sb + a4 * (Cfg::kBBytes / 4), tb, &full_bar[stage], bcol0 + a4 * 64, kb * kBlockK);
+            } else {
+              // segmented K rows (TN form, 3-D map): K row g -> (segment g / seg_rows, row g % seg_rows); seg_rows is a multiple of
+              // 64, so a k-block never straddles two segments (576 = 9 x 64: one crop of a [:,1:] CLIP hidden state)
+              const int g = kb * kBlockK;
+              const int seg = g / pr.b_seg_rows;
+#pragma unroll
+              for (int a4 = 0; a4 < 4; ++a4)
+                tma_load_3d(sb + a4 * (Cfg::kBBytes / 4), tb, &full_bar[stage], bcol0 + a4 * 64, g - seg * pr.b_seg_rows, seg);
+            }
           }
         }
         __syncwarp();

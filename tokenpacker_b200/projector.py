@@ -39,6 +39,23 @@ def _two_layer(in_dim: int, mid: int, out: int) -> nn.Sequential:
     return nn.Sequential(nn.Linear(in_dim, mid), nn.GELU(), nn.Linear(mid, out))
 
 
+def _pack_train(module, params, device):
+    """(bf16 parameters, their tp_weights, packed weights) for one training step."""
+    # training: ALWAYS repack from the live parameters.  Optimizers that update through a ``.data`` alias (DeepSpeed ZeRO-2's
+    # bit16 flat buffer: every reference recipe, scripts/v1_5/*.sh) change neither data_ptr nor _version, so no key can tell
+    # that the weights moved; they change every step anyway and the pack is small next to forward + backward.
+    # The matrices that need no transformation are read from the (bf16) parameters in place; only the fp32 biases, the
+    # LayerNorm-folded in-projections and the k/v_proj.0 concatenation are rebuilt (tp_pack_weights_train).
+    bf = [p.detach().to(device=device, dtype=torch.bfloat16).contiguous() for p in params]
+    w_struct = _lib.TpWeights(*[t.data_ptr() for t in bf])
+    stream = torch.cuda.current_stream(device).cuda_stream
+    pbytes = lib.tp_packed_bytes(module.hidden_size)
+    packed = torch.empty(pbytes, dtype=torch.uint8, device=device)
+    check(lib.tp_pack_weights_train(C.byref(w_struct), module.hidden_size, packed.data_ptr(), pbytes, stream), "tp_pack_weights_train")
+    module._packed = module._packed_key = None           # whatever the inference path cached predates this step's weights
+    return bf, w_struct, packed
+
+
 class _ProjectorFunction(torch.autograd.Function):
     """autograd bridge: forward = tp_forward_train (keeps intermediates), backward = tp_backward (parameter gradients), or
     tp_backward_inputs when x0b / xmb need a gradient too (``TokenPackerB200.input_grad``)."""
@@ -47,18 +64,8 @@ class _ProjectorFunction(torch.autograd.Function):
     def forward(ctx, module, x0b, s0, xmb, sm, *params):
         device = x0b.device
         n = x0b.shape[0]
-        # training: ALWAYS repack from the live parameters.  Optimizers that update through a ``.data`` alias (DeepSpeed ZeRO-2's
-        # bit16 flat buffer: every reference recipe, scripts/v1_5/*.sh) change neither data_ptr nor _version, so no key can tell
-        # that the weights moved; they change every step anyway and the pack is small next to forward + backward.
-        # The matrices that need no transformation are read from the (bf16) parameters in place; only the fp32 biases, the
-        # LayerNorm-folded in-projections and the k/v_proj.0 concatenation are rebuilt (tp_pack_weights_train).
-        bf = [p.detach().to(device=device, dtype=torch.bfloat16).contiguous() for p in params]
-        w_struct = _lib.TpWeights(*[t.data_ptr() for t in bf])
+        bf, w_struct, packed = _pack_train(module, params, device)
         stream = torch.cuda.current_stream(device).cuda_stream
-        pbytes = lib.tp_packed_bytes(module.hidden_size)
-        packed = torch.empty(pbytes, dtype=torch.uint8, device=device)
-        check(lib.tp_pack_weights_train(C.byref(w_struct), module.hidden_size, packed.data_ptr(), pbytes, stream), "tp_pack_weights_train")
-        module._packed = module._packed_key = None           # whatever the inference path cached predates this step's weights
         out = torch.empty((n, module.num_queries, module.hidden_size), dtype=torch.bfloat16, device=device)
         nbytes = lib.tp_train_saved_bytes(n, module.scale_factor, module.hidden_size)
         saved = torch.empty(nbytes, dtype=torch.uint8, device=device)
@@ -100,6 +107,68 @@ class _ProjectorFunction(torch.autograd.Function):
                                       g.data_ptr(), ctx.saved.data_ptr(), C.byref(g_struct), ws.data_ptr(), ws_bytes, stream), "tp_backward")
         out = [gr.to(dt) if need else None for gr, (dt, need) in zip(grads, ctx.param_meta)]
         return (None, d_x0, None, d_xm, None) + tuple(out)
+
+
+def _token_rows(layers):
+    """ctypes array of the four layers' token row 0 (after the CLS row of a [N,577,1024] layer)."""
+    return (C.c_void_p * 4)(*[t.data_ptr() + (t.shape[1] - 576) * 1024 * t.element_size() for t in layers])
+
+
+class _HiddenStatesFunction(torch.autograd.Function):
+    """autograd bridge of ``TokenPackerB200.forward_hidden_states``: forward = tp_forward_train_layers, backward = tp_backward_layers,
+    both reading the four bf16 hidden states (each [N,577,1024] or each [N,576,1024], one crop stride) in place.  Layer gradients
+    come back in the layers' shape, CLS rows zero, written by the backward's GEMMs straight into their token rows."""
+
+    @staticmethod
+    def forward(ctx, module, l0, l1, l2, l3, *params):
+        layers = (l0, l1, l2, l3)
+        device = l0.device
+        n = l0.shape[0]
+        bf, w_struct, packed = _pack_train(module, params, device)
+        stream = torch.cuda.current_stream(device).cuda_stream
+        out = torch.empty((n, module.num_queries, module.hidden_size), dtype=torch.bfloat16, device=device)
+        nbytes = lib.tp_train_saved_bytes(n, module.scale_factor, module.hidden_size)
+        saved = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        check(lib.tp_forward_train_layers(C.byref(w_struct), packed.data_ptr(), _token_rows(layers), n, l0.stride(0), module.scale_factor,
+                                          module.hidden_size, out.data_ptr(), saved.data_ptr(), nbytes, stream), "tp_forward_train_layers")
+        ctx.module = module
+        ctx.saved = saved
+        ctx.packed = packed if any(ctx.needs_input_grad[1:5]) else None   # the layer gradients read [W_k0; W_v0] from it
+        ctx.weights_bf16 = bf
+        ctx.param_meta = [(p.dtype, p.requires_grad) for p in params]
+        ctx.save_for_backward(*layers)                       # read again by the backward: an in-place edit before it raises
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        module = ctx.module
+        layers = ctx.saved_tensors
+        device = grad_out.device
+        n, rows = layers[0].shape[0], layers[0].shape[1]
+        g = grad_out.to(torch.bfloat16).contiguous()
+        grads = [torch.empty_like(w) for w in ctx.weights_bf16]
+        w_struct = _lib.TpWeights(*[t.data_ptr() for t in ctx.weights_bf16])
+        g_struct = _lib.TpWeights(*[t.data_ptr() for t in grads])
+        need = ctx.needs_input_grad[1:5]
+        d = [None] * 4
+        with torch.cuda.device(device):
+            d_ptrs = None
+            if any(need):
+                for i in range(4):
+                    if need[i]:
+                        d[i] = torch.empty((n, rows, 1024), dtype=torch.bfloat16, device=device)     # token rows: every element written
+                        if rows == 577:
+                            d[i][:, 0].zero_()
+                d_ptrs = (C.c_void_p * 4)(*[t.data_ptr() + (rows - 576) * 2048 if t is not None else None for t in d])
+            ws_bytes = lib.tp_backward_workspace_bytes(n, module.scale_factor, module.hidden_size)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+            stream = torch.cuda.current_stream(device).cuda_stream
+            check(lib.tp_backward_layers(C.byref(w_struct), ctx.packed.data_ptr() if ctx.packed is not None else None, _token_rows(layers),
+                                         layers[0].stride(0), n, module.scale_factor, module.hidden_size, g.data_ptr(), ctx.saved.data_ptr(),
+                                         C.byref(g_struct), d_ptrs, rows * 1024, ws.data_ptr(), ws_bytes, stream), "tp_backward_layers")
+        out = [gr.to(dt) if need_p else None for gr, (dt, need_p) in zip(grads, ctx.param_meta)]
+        return (None, *d) + tuple(out)
 
 
 class _PackedScatterFunction(torch.autograd.Function):
@@ -341,6 +410,96 @@ class TokenPackerB200(nn.Module):
             check(lib.tp_forward_layers(packed.data_ptr(), arr, n, stride, self.scale_factor, self.hidden_size, out.data_ptr(), None,
                                         ws.data_ptr(), ws_bytes, stream), "tp_forward_layers")
         return out
+
+    def _check_layers(self, layers):
+        if not isinstance(layers, (tuple, list)) or len(layers) != 4:
+            raise ValueError("expected the 4 hidden states (12, 16, 22, 23)")
+        for t in layers:
+            if not isinstance(t, torch.Tensor) or t.dim() != 3 or t.shape[2] != 1024 or t.shape[1] not in (576, 577) \
+                    or t.shape[0] != layers[0].shape[0]:
+                raise ValueError("each layer must be a tensor [N,577,1024] or [N,576,1024], with the same N")
+        if torch.is_grad_enabled() and any(t.requires_grad for t in layers) and not self.input_grad:
+            raise NotImplementedError("gradients w.r.t. the CLIP hidden states are off by default (the vision tower is frozen in every "
+                                      "released TokenPacker recipe): set `projector.input_grad = True` to have forward_hidden_states() "
+                                      "produce them, or detach the layers or run under torch.no_grad()")
+        if not all(t.is_cuda for t in layers):
+            raise RuntimeError("tokenpacker_b200 has no CPU path: inputs must be CUDA tensors on an H100")
+        return list(layers)
+
+    @staticmethod
+    def _hidden_state_operands(layers):
+        """(bases, token views, crop stride): when the four layers are bf16 of one shape whose token rows share a TMA-compatible crop
+        stride (the tower's own [N,577,1024] outputs), bases are the layers themselves and nothing is copied; else bases = views =
+        contiguous bf16 [N,576,1024] copies, whose cast / slice backward autograd carries."""
+        if all(t.dtype == torch.bfloat16 for t in layers) and len({t.shape[1] for t in layers}) == 1:
+            views = [t[:, 1:] if t.shape[1] == 577 else t for t in layers]
+            stride = views[0].stride(0)
+            if stride % 8 == 0 and stride >= 576 * 1024 and all(v.stride(2) == 1 and v.stride(1) == 1024 and v.stride(0) == stride
+                                                                and v.data_ptr() % 16 == 0 for v in views):
+                return list(layers), views, stride
+        views = [(t[:, 1:] if t.shape[1] == 577 else t).to(torch.bfloat16).contiguous() for t in layers]
+        return views, views, views[0].stride(0)
+
+    def _hidden_states_train(self, layers) -> bool:
+        return torch.is_grad_enabled() and (any(p.requires_grad for p in self._raw_params()) or
+                                            (self.input_grad and any(t.requires_grad for t in layers)))
+
+    def forward_hidden_states(self, layers):
+        """Forward from the four CLIP hidden states (layers 12, 16, 22, 23: ``hidden_states[l]`` of the tower, each [N,577,1024] with
+        the CLS row or [N,576,1024]) -> [N, M, hidden]: ``feature_select`` + ``torch.cat`` (clip_encoder.py:28-44) + ``forward``
+        without the concatenation.  Differentiable: under autograd the training kernels read the layers in place (no concatenated or
+        copied feat_multi is ever made) and, with ``input_grad``, give each layer its gradient (layer 23's is the sum of its feat and
+        feat_multi paths), in the layer's shape and dtype with zero CLS rows.  Without gradients this is ``forward_layers``."""
+        layers = self._check_layers(layers)
+        out_dtype = layers[3].dtype
+        if layers[0].shape[0] == 0:
+            return layers[3].new_empty((0, self.num_queries, self.hidden_size))
+        if not self._hidden_states_train(layers):
+            out = self.forward_layers(layers)
+        else:
+            with torch.cuda.device(layers[0].device):
+                bases, _, _ = self._hidden_state_operands(layers)
+                out = _HiddenStatesFunction.apply(self, *bases, *self._raw_params())
+        return out if out_dtype == torch.bfloat16 else out.to(out_dtype)
+
+    def forward_hidden_states_packed(self, layers, h_block, w_block, sep_row, ret_row):
+        """``forward_packed`` from the four CLIP hidden states (as in ``forward_hidden_states``): projector + HD slice assembly
+        (llava_arch.py:139-155).  Inference: the last GEMM's TMA stores write the packed rows directly (tp_forward_layers_packed) and a
+        tiny kernel fills the separator rows.  Under autograd: ``forward_hidden_states`` plus the differentiable scatter.  Returns
+        (packed [sum(L_i), hidden], cu_seqlens int64 [B+1] on the host)."""
+        from .hd import hd_plan_device
+        layers = self._check_layers(layers)
+        device = layers[0].device
+        n = layers[0].shape[0]
+        plan, seg, sep_rows, ret_rows = hd_plan_device(h_block, w_block, self.num_queries, device)
+        if plan.n_crops != n:
+            raise ValueError(f"grids describe {plan.n_crops} crops but {n} were given")
+        total = int(plan.cu_seqlens[-1])
+        crop_rows = self.num_queries + 1
+        assert total == plan.n_crops * crop_rows      # one separator row per crop: the uniform stride the kernel relies on
+        training = self._hidden_states_train(layers) or (torch.is_grad_enabled() and (sep_row.requires_grad or ret_row.requires_grad))
+        with torch.cuda.device(device):
+            if training:
+                feats = self.forward_hidden_states(layers).to(torch.bfloat16)
+                out = _PackedScatterFunction.apply(feats, sep_row, ret_row, seg, sep_rows, ret_rows, total)
+            else:
+                with torch.no_grad():
+                    _, views, stride = self._hidden_state_operands(layers)
+                    packed = self._packed_weights(device)
+                    out = torch.empty((total, self.hidden_size), dtype=torch.bfloat16, device=device)
+                    ws_bytes = lib.tp_workspace_bytes(n, self.scale_factor, self.hidden_size)
+                    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+                    stream = torch.cuda.current_stream(device).cuda_stream
+                    arr = (C.c_void_p * 4)(*[v.data_ptr() for v in views])
+                    check(lib.tp_forward_layers_packed(packed.data_ptr(), arr, n, stride, self.scale_factor, self.hidden_size,
+                                                       out.data_ptr(), crop_rows, ws.data_ptr(), ws_bytes, stream), "tp_forward_layers_packed")
+                    sep_b = sep_row.to(device=device, dtype=torch.bfloat16).contiguous()
+                    ret_b = ret_row.to(device=device, dtype=torch.bfloat16).contiguous()
+                    check(lib.tp_hd_fill_separators(out.data_ptr(), self.hidden_size, sep_rows.data_ptr(), sep_rows.numel(),
+                                                    sep_b.data_ptr(), ret_rows.data_ptr(), ret_rows.numel(), ret_b.data_ptr(), stream),
+                          "tp_hd_fill_separators")
+        out_dtype = layers[3].dtype
+        return (out if out_dtype == torch.bfloat16 else out.to(out_dtype)), plan.cu_seqlens
 
     def _require_inference(self, what: str):
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
