@@ -810,6 +810,15 @@ int launch_attn_s(int s, const __nv_bfloat16* qp, const __nv_bfloat16* kp, const
   }
 }
 
+// out[c, r] = in[r, c]  (in: [rows, cols] bf16, row stride ld_in; out: [cols, rows], row stride ld_out)
+int launch_transpose(const void* in, long long ld_in, void* out, long long ld_out, long long rows, int cols, cudaStream_t stream) {
+  const dim3 grid(static_cast<unsigned>((cols + 31) / 32), static_cast<unsigned>((rows + 31) / 32));
+  transpose_kernel<<<grid, dim3(32, 8), 0, stream>>>(static_cast<const __nv_bfloat16*>(in), ld_in, static_cast<__nv_bfloat16*>(out), ld_out, rows,
+                                                      cols);
+  TP_CUDA(cudaGetLastError()); ++g_launch_count;
+  return TP_OK;
+}
+
 }  // namespace
 
 // ==================================================================================================
@@ -837,68 +846,6 @@ const char* tp_last_cuda_error(void) { return g_last_cuda_error; }
 uint64_t tp_launch_count(void) { return g_launch_count.load(std::memory_order_relaxed); }
 
 size_t tp_packed_bytes(int hidden) { return valid_hidden(hidden) ? packed_layout(hidden).total : 0; }
-
-int tp_pack_weights(const tp_weights* w, int hidden, void* packed, size_t packed_bytes, void* stream_) {
-  if (w == nullptr || packed == nullptr || !valid_hidden(hidden)) return TP_ERR_INVALID_ARGUMENT;
-  const void* const* fields = reinterpret_cast<const void* const*>(w);
-  for (size_t i = 0; i < sizeof(tp_weights) / sizeof(void*); ++i)
-    if (fields[i] == nullptr) return TP_ERR_INVALID_ARGUMENT;
-  const PackedLayout L = packed_layout(hidden);
-  if (packed_bytes < L.total) return TP_ERR_WORKSPACE_TOO_SMALL;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  uint8_t* P = static_cast<uint8_t*>(packed);
-  const size_t mat = static_cast<size_t>(kC) * kC * 2;
-  auto copy = [&](size_t off, const void* src, size_t bytes) { return cudaMemcpyAsync(P + off, src, bytes, cudaMemcpyDeviceToDevice, stream); };
-  auto bias = [&](size_t off, const void* src, int n) {
-    bf16_to_f32_kernel<<<(n + 255) / 256, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(src), reinterpret_cast<float*>(P + off), n);
-    return cudaGetLastError();
-  };
-  auto fold = [&](size_t w_off, size_t wsum_off, size_t c_off, const void* wsrc, const void* bsrc, const void* gamma, const void* beta) {
-    fold_layernorm_kernel<<<(kC * 32 + 255) / 256, 256, 0, stream>>>(
-        static_cast<const __nv_bfloat16*>(wsrc), static_cast<const __nv_bfloat16*>(bsrc), static_cast<const __nv_bfloat16*>(gamma),
-        static_cast<const __nv_bfloat16*>(beta), reinterpret_cast<__nv_bfloat16*>(P + w_off), reinterpret_cast<float*>(P + wsum_off),
-        reinterpret_cast<float*>(P + c_off), kC, kC);
-    return cudaGetLastError();
-  };
-  const size_t kv0 = static_cast<size_t>(kC) * kCm * 2;
-  TP_CUDA(copy(L.w_kv0, w->k_proj_0_w, kv0));
-  TP_CUDA(copy(L.w_kv0 + kv0, w->v_proj_0_w, kv0));
-  TP_CUDA(bias(L.b_kv0, w->k_proj_0_b, kC));
-  TP_CUDA(bias(L.b_kv0 + kC * 4, w->v_proj_0_b, kC));
-  TP_CUDA(copy(L.w_k2, w->k_proj_2_w, mat));
-  TP_CUDA(bias(L.b_k2, w->k_proj_2_b, kC));
-  TP_CUDA(copy(L.w_v2, w->v_proj_2_w, mat));
-  TP_CUDA(bias(L.b_v2, w->v_proj_2_b, kC));
-  const __nv_bfloat16* in_w = static_cast<const __nv_bfloat16*>(w->in_proj_w);
-  const __nv_bfloat16* in_b = static_cast<const __nv_bfloat16*>(w->in_proj_b);
-  // clip_attn.in_proj_weight rows [0,C) = q, [C,2C) = k, [2C,3C) = v   (torch MHA packed in-projection)
-  TP_CUDA(fold(L.w_iq, L.wsum_q, L.c_q, in_w, in_b, w->ln_q_w, w->ln_q_b));
-  TP_CUDA(fold(L.w_ik, L.wsum_k, L.c_k, in_w + static_cast<size_t>(kC) * kC, in_b + kC, w->ln_k_w, w->ln_k_b));
-  TP_CUDA(fold(L.w_iv, L.wsum_v, L.c_v, in_w + 2 * static_cast<size_t>(kC) * kC, in_b + 2 * kC, w->ln_v_w, w->ln_v_b));
-  TP_CUDA(copy(L.w_q, w->q_proj_w, mat));
-  // out_proj folded into mlp.0 (exact re-association, no nonlinearity in between):
-  //   mlp.0(out_proj(x)) = (W_m0 W_o) x + (W_m0 b_o + b_m0);  W_m0 W_o computed by our own GEMM with B = W_o^T (K-major)
-  {
-    DeviceInfo dev;
-    TP_TRY(device_info(&dev));
-    transpose_bf16_kernel<<<dim3(kC / 32, kC / 32), dim3(32, 8), 0, stream>>>(static_cast<const __nv_bfloat16*>(w->out_proj_w),
-                                                                              reinterpret_cast<__nv_bfloat16*>(P + L.w_ot), kC);
-    TP_CUDA(cudaGetLastError()); ++g_launch_count;
-    TP_TRY(launch_gemm(AOperand{w->mlp_0_w, kC, 0, 0}, P + L.w_ot, kC, hidden, kC, kC, plain_epilogue(P + L.w_om, kC, nullptr, 0), dev.sms, stream));
-    matvec_bias_kernel<<<(hidden * 32 + 255) / 256, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(w->mlp_0_w),
-                                                                      static_cast<const __nv_bfloat16*>(w->out_proj_b),
-                                                                      static_cast<const __nv_bfloat16*>(w->mlp_0_b),
-                                                                      reinterpret_cast<float*>(P + L.b_om), hidden, kC);
-    TP_CUDA(cudaGetLastError()); ++g_launch_count;
-  }
-  TP_CUDA(copy(L.w_o, w->out_proj_w, mat));
-  TP_CUDA(bias(L.b_o, w->out_proj_b, kC));
-  TP_CUDA(copy(L.w_m0, w->mlp_0_w, static_cast<size_t>(hidden) * kC * 2));
-  TP_CUDA(bias(L.b_m0, w->mlp_0_b, hidden));
-  TP_CUDA(copy(L.w_m2, w->mlp_2_w, static_cast<size_t>(hidden) * hidden * 2));
-  TP_CUDA(bias(L.b_m2, w->mlp_2_b, hidden));
-  return TP_OK;
-}
 
 int tp_pack_weights_train(const tp_weights* w, int hidden, void* packed, size_t packed_bytes, void* stream_) {
   if (w == nullptr || packed == nullptr || !valid_hidden(hidden)) return TP_ERR_INVALID_ARGUMENT;
@@ -936,9 +883,35 @@ int tp_pack_weights_train(const tp_weights* w, int hidden, void* packed, size_t 
     ++g_launch_count;
     return cudaGetLastError();
   };
+  // clip_attn.in_proj_weight rows [0,C) = q, [C,2C) = k, [2C,3C) = v   (torch MHA packed in-projection)
   TP_CUDA(fold(L.w_iq, L.wsum_q, L.c_q, in_w, in_b, w->ln_q_w, w->ln_q_b));
   TP_CUDA(fold(L.w_ik, L.wsum_k, L.c_k, in_w + static_cast<size_t>(kC) * kC, in_b + kC, w->ln_k_w, w->ln_k_b));
   TP_CUDA(fold(L.w_iv, L.wsum_v, L.c_v, in_w + 2 * static_cast<size_t>(kC) * kC, in_b + 2 * kC, w->ln_v_w, w->ln_v_b));
+  return TP_OK;
+}
+
+// Everything tp_pack_weights_train packs, and what only the inference forward reads: the weights it uses unchanged, and out_proj folded
+// into mlp.0 (exact re-association, no nonlinearity in between):
+//   mlp.0(out_proj(x)) = (W_m0 W_o) x + (W_m0 b_o + b_m0);  W_m0 W_o computed by our own GEMM with B = W_o^T (K-major)
+int tp_pack_weights(const tp_weights* w, int hidden, void* packed, size_t packed_bytes, void* stream_) {
+  TP_TRY(tp_pack_weights_train(w, hidden, packed, packed_bytes, stream_));
+  const PackedLayout L = packed_layout(hidden);
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  uint8_t* P = static_cast<uint8_t*>(packed);
+  const size_t mat = static_cast<size_t>(kC) * kC * 2;
+  const struct { size_t off; const void* src; size_t bytes; } copies[] = {
+      {L.w_k2, w->k_proj_2_w, mat}, {L.w_v2, w->v_proj_2_w, mat}, {L.w_q, w->q_proj_w, mat}, {L.w_o, w->out_proj_w, mat},
+      {L.w_m0, w->mlp_0_w, static_cast<size_t>(hidden) * kC * 2}, {L.w_m2, w->mlp_2_w, static_cast<size_t>(hidden) * hidden * 2}};
+  for (const auto& c : copies) TP_CUDA(cudaMemcpyAsync(P + c.off, c.src, c.bytes, cudaMemcpyDeviceToDevice, stream));
+  DeviceInfo dev;
+  TP_TRY(device_info(&dev));
+  TP_TRY(launch_transpose(w->out_proj_w, kC, P + L.w_ot, kC, kC, kC, stream));
+  TP_TRY(launch_gemm(AOperand{w->mlp_0_w, kC, 0, 0}, P + L.w_ot, kC, hidden, kC, kC, plain_epilogue(P + L.w_om, kC, nullptr, 0), dev.sms, stream));
+  matvec_bias_kernel<<<(hidden * 32 + 255) / 256, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(w->mlp_0_w),
+                                                                    static_cast<const __nv_bfloat16*>(w->out_proj_b),
+                                                                    static_cast<const __nv_bfloat16*>(w->mlp_0_b),
+                                                                    reinterpret_cast<float*>(P + L.b_om), hidden, kC);
+  TP_CUDA(cudaGetLastError()); ++g_launch_count;
   return TP_OK;
 }
 
@@ -955,9 +928,9 @@ namespace {
 // ~100 cuTensorMapEncodeTiled calls and replays the stored launch.  Per host thread, 4 entries, round-robin replacement.  (TP_FUSE_ATTN,
 // TP_CHAIN and TP_GEMM_MODE only decide whether this plan runs at all, and are read before the cache is probed.)
 struct FwdKey {
-  const void* packed; const void* x0; const void* xm; const void* layers[4]; void* out; void* ws; const void* peers[kMaxPeers];
+  const void* packed; const void* x0; const void* xm[4]; void* out; void* ws; const void* peers[kMaxPeers];
   long long n, s0, sm, crop_rows;
-  int s, H, n_peers, sms;
+  int s, H, n_peers, sms, parts;
 };
 struct FwdPlan {
   FwdKey key;
@@ -978,25 +951,99 @@ int check_layers(const void* const* layers, int64_t crop_stride) {
   return TP_OK;
 }
 
-// xm_layers != nullptr: the multi-level stack is given as its four [n_crops, 576, 1024] layers (row stride 1024, crop stride
-// xm_crop_stride) instead of one [n_crops, 576, 4096] tensor; ``xm`` is then ignored.
-int forward_impl(const void* packed, const void* x0, const void* xm, const void* const* xm_layers, int64_t n_crops, int64_t x0_crop_stride,
-                 int64_t xm_crop_stride, int scale_factor, int hidden, void* out, const int64_t* seg_row_offset, int64_t out_crop_rows,
-                 void* const* peer_out, int n_peers, void* workspace, size_t workspace_bytes, void* stream_) {
-  if (xm_layers != nullptr) {
-    for (int i = 0; i < 4; ++i)
-      if (xm_layers[i] == nullptr) return TP_ERR_INVALID_ARGUMENT;
-    xm = xm_layers[0];
+// What the forward and the backward read from the CLIP tower: feat, and the multi-level stack either as one [n_crops, 576, 4096]
+// concatenation (parts = 1) or as its four [n_crops, 576, 1024] layers side by side (parts = 4), crops xm_crop_stride elements apart.
+// The k/v_proj.0 GEMMs read the four layers in place as four parts of one operand: each walks the same k-blocks (forward) or output
+// tiles (weight gradient) in the same order as the concatenation, so both forms give the same bits.  Only the methods below branch on
+// the form.
+struct Features {
+  const void* x0;
+  int64_t x0_crop_stride;
+  const void* xm[4];        // the concatenation, or the four layers
+  int64_t xm_crop_stride;
+  int parts;
+
+  static Features cat(const void* x0, int64_t x0_crop_stride, const void* xm, int64_t xm_crop_stride) {
+    return Features{x0, x0_crop_stride, {xm, nullptr, nullptr, nullptr}, xm_crop_stride, 1};
   }
+  // the four hidden states of include/tokenpacker_b200_layers.h: the last one is feat as well
+  static Features layers(const void* const* l, int64_t crop_stride) {
+    return Features{l[3], crop_stride, {l[0], l[1], l[2], l[3]}, crop_stride, 4};
+  }
+  long long ld() const { return kCm / parts; }
+  // both operands given, crops at least 576 rows apart and a 16-byte multiple apart (TMA strides)
+  bool valid() const {
+    return x0 != nullptr && xm[0] != nullptr && x0_crop_stride >= static_cast<int64_t>(kTokens) * kC && x0_crop_stride % 8 == 0 &&
+           xm_crop_stride >= kTokens * ld() && xm_crop_stride % 8 == 0;
+  }
+  // A of stage [1] (xm [W_k0; W_v0]^T): crop-strided rows are a 3-D [n_crops, 576, K] operand
+  AOperand stage1_a() const {
+    AOperand a{xm[0], ld(), 0, 0};
+    if (xm_crop_stride != kTokens * ld()) a = AOperand{xm[0], ld(), kTokens, xm_crop_stride};
+    a.parts = parts;
+    for (int i = 1; i < 4; ++i) a.more[i - 1] = xm[i];
+    return a;
+  }
+  // The concatenation is the k/v_proj.0 weight gradients' B operand as one plain [R, 4096] matrix, so its crops must be contiguous;
+  // the layers are read crop-strided.
+  bool wgrad_b_ok() const { return parts == 4 || xm_crop_stride == static_cast<int64_t>(kTokens) * kCm; }
+  // B of those weight gradients: the four layers side by side along N, K rows = tokens in 576-row crops
+  void set_wgrad_b(GemmItem* it) const {
+    it->b = xm[0];
+    it->ldb = ld();
+    if (parts == 1) return;
+    it->b_parts = parts;
+    for (int i = 1; i < 4; ++i) it->b_more[i - 1] = xm[i];
+    it->b_seg_rows = kTokens;
+    it->b_seg_stride = xm_crop_stride;
+  }
+};
+
+// The forward's buffers that stages [1] - [3] write and read: the inference workspace, or the activations the training forward saves
+struct StageBufs {
+  __nv_bfloat16 *h_kv, *q, *y_k, *y_v, *y_q, *k_p, *v_p, *q_p;
+  float *stats_k, *stats_v, *stats_q;
+};
+
+// it[0] = [1] h_kv = GELU(xm [W_k0; W_v0]^T + b); it[1..3] = [2] y_k | y_v | y_q = the second linears of k / v and q_proj_1, each
+// storing its rows' LayerNorm statistics.  Their weights are the live parameters when w != NULL, else the packed copies.
+void stage12_items(GemmItem* it, const Features& f, const uint8_t* P, const PackedLayout& L, const tp_weights* w, const StageBufs& b,
+                   long long R, long long Q) {
+  auto wf = [&](size_t off) { return reinterpret_cast<const float*>(P + off); };
+  it[0] = GemmItem{f.stage1_a(), P + L.w_kv0, kCm, R, 2 * kC, kCm, plain_epilogue(b.h_kv, 2 * kC, wf(L.b_kv0), 1)};
+  it[1] = GemmItem{AOperand{b.h_kv, 2 * kC, 0, 0}, w != nullptr ? w->k_proj_2_w : P + L.w_k2, kC, R, kC, kC,
+                   plain_epilogue(b.y_k, kC, wf(L.b_k2), 0)};
+  it[1].ep.stats_out = b.stats_k;
+  it[2] = GemmItem{AOperand{b.h_kv + kC, 2 * kC, 0, 0}, w != nullptr ? w->v_proj_2_w : P + L.w_v2, kC, R, kC, kC,
+                   plain_epilogue(b.y_v, kC, wf(L.b_v2), 0)};
+  it[2].ep.stats_out = b.stats_v;
+  it[3] = GemmItem{AOperand{b.q, kC, 0, 0}, w != nullptr ? w->q_proj_w : P + L.w_q, kC, Q, kC, kC, plain_epilogue(b.y_q, kC, nullptr, 0)};
+  it[3].ep.stats_out = b.stats_q;
+  for (int i = 1; i <= 3; ++i) it[i].ep.stats_out_slots = kStatSlots;
+}
+
+// it[0..2] = [3] k' | v' | q' = the LayerNorms folded into the MHA in-projections (q' scaled by 1/sqrt 128)
+void stage3_items(GemmItem* it, const uint8_t* P, const PackedLayout& L, const StageBufs& b, long long R, long long Q) {
+  auto wf = [&](size_t off) { return reinterpret_cast<const float*>(P + off); };
+  it[0] = GemmItem{AOperand{b.y_k, kC, 0, 0}, P + L.w_ik, kC, R, kC, kC, plain_epilogue(b.k_p, kC, wf(L.c_k), 0)};
+  it[0].ep.col_a = wf(L.wsum_k);
+  it[0].ep.stats_in = b.stats_k;
+  it[1] = GemmItem{AOperand{b.y_v, kC, 0, 0}, P + L.w_iv, kC, R, kC, kC, plain_epilogue(b.v_p, kC, wf(L.c_v), 0)};
+  it[1].ep.col_a = wf(L.wsum_v);
+  it[1].ep.stats_in = b.stats_v;
+  it[2] = GemmItem{AOperand{b.y_q, kC, 0, 0}, P + L.w_iq, kC, Q, kC, kC, plain_epilogue(b.q_p, kC, wf(L.c_q), 0)};
+  it[2].ep.col_a = wf(L.wsum_q);
+  it[2].ep.stats_in = b.stats_q;
+  it[2].ep.alpha = 0.08838834764831845f;   // 1/sqrt(head_dim = 128): torch MHA scales q after the in-projection
+  for (int i = 0; i < 3; ++i) it[i].ep.stats_in_slots = kStatSlots;
+}
+
+int forward_impl(const void* packed, const Features& f, int64_t n_crops, int scale_factor, int hidden, void* out, const int64_t* seg_row_offset,
+                 int64_t out_crop_rows, void* const* peer_out, int n_peers, void* workspace, size_t workspace_bytes, void* stream_) {
   if (scale_factor <= 0 || kGrid % scale_factor != 0) return TP_ERR_BAD_SCALE_FACTOR;          // builder.py:51-52
-  if (packed == nullptr || x0 == nullptr || xm == nullptr || out == nullptr || workspace == nullptr || n_crops <= 0 ||
-      !valid_hidden(hidden))
+  if (packed == nullptr || !f.valid() || out == nullptr || workspace == nullptr || n_crops <= 0 || !valid_hidden(hidden) ||
+      n_crops * kTokens > 0x7fff0000ll)
     return TP_ERR_INVALID_ARGUMENT;
-  const int64_t xm_width = xm_layers != nullptr ? kC : kCm;
-  if (x0_crop_stride < static_cast<int64_t>(kTokens) * kC || xm_crop_stride < static_cast<int64_t>(kTokens) * xm_width ||
-      x0_crop_stride % 8 != 0 || xm_crop_stride % 8 != 0)
-    return TP_ERR_INVALID_ARGUMENT;
-  if (n_crops * kTokens > 0x7fff0000ll) return TP_ERR_INVALID_ARGUMENT;
   DeviceInfo dev;
   TP_TRY(device_info(&dev));
   const int s = scale_factor, H = hidden;
@@ -1011,9 +1058,12 @@ int forward_impl(const void* packed, const void* x0, const void* xm, const void*
   auto wf = [&](size_t off) { return reinterpret_cast<const float*>(P + off); };
   auto bf = [&](size_t off) { return reinterpret_cast<__nv_bfloat16*>(ws + off); };
 
-  float* stats_k = reinterpret_cast<float*>(ws + W.stats);
-  float* stats_v = stats_k + 2 * kStatSlots * R;
-  float* stats_q = stats_v + 2 * kStatSlots * R;     // every slot is written by the producing GEMM: no memset needed
+  // k' / v' have buffers of their own: in a chained launch [3] runs while other row blocks of [2] still read h_kv, so the
+  // round-1 trick of writing them over the dead h_kv buffer is no longer legal
+  StageBufs bufs{bf(W.h_kv), bf(W.q), bf(W.y_k), bf(W.y_v), bf(W.y_q), bf(W.k_p), bf(W.v_p), bf(W.q_p)};
+  bufs.stats_k = reinterpret_cast<float*>(ws + W.stats);
+  bufs.stats_v = bufs.stats_k + 2 * kStatSlots * R;
+  bufs.stats_q = bufs.stats_v + 2 * kStatSlots * R;     // every slot is written by the producing GEMM: no memset needed
 
   // Launch plan.  Large batches: 4 launches — [S], chain A = {[1], [2], [3]} and chain B = {[4], [5]} as ONE persistent CTA-pair
   // launch each (stages ordered by per-row-block tile counters instead of kernel boundaries), [A] in between.  Small batches
@@ -1030,9 +1080,9 @@ int forward_impl(const void* packed, const void* x0, const void* xm, const void*
   TP_CUDA(cudaMemsetAsync(flags, 0, static_cast<size_t>(W.n_flags) * 4, stream));      // tile counters of the chained launches
   FrontWork front;
   memset(&front, 0, sizeof(front));
-  front.x0 = static_cast<const __nv_bfloat16*>(x0);
-  front.q = bf(W.q);
-  front.crop_stride = x0_crop_stride;
+  front.x0 = static_cast<const __nv_bfloat16*>(f.x0);
+  front.q = bufs.q;
+  front.crop_stride = f.x0_crop_stride;
   front.n_queries = Q;
   front.s = s;
   // ---- fully fused plan (scale factors 2 and 4, batches large enough for pair tiles): ONE launch for the whole forward.
@@ -1042,32 +1092,14 @@ int forward_impl(const void* packed, const void* x0, const void* xm, const void*
   const char* fuse_env = getenv("TP_FUSE_ATTN");       // A/B aid, read per call: TP_FUSE_ATTN=0 -> separate attention kernel
   const bool fuse_off = fuse_env != nullptr && atoi(fuse_env) == 0;
   if ((s == 2 || s == 4) && !fuse_off && seg_row_offset == nullptr) {
-    GemmItem g[8];
-    AOperand a{xm, xm_width, 0, 0};
-    if (xm_crop_stride != static_cast<int64_t>(kTokens) * xm_width) a = AOperand{xm, xm_width, kTokens, xm_crop_stride};
-    if (xm_layers != nullptr) {
-      a.parts = 4;
-      for (int i = 1; i < 4; ++i) a.more[i - 1] = xm_layers[i];
-    }
-    g[0] = GemmItem{a, P + L.w_kv0, kCm, R, 2 * kC, kCm, plain_epilogue(bf(W.h_kv), 2 * kC, wf(L.b_kv0), 1)};
-    g[1] = GemmItem{AOperand{bf(W.h_kv), 2 * kC, 0, 0}, P + L.w_k2, kC, R, kC, kC, plain_epilogue(bf(W.y_k), kC, wf(L.b_k2), 0)};
-    g[1].ep.stats_out = stats_k;
-    g[2] = GemmItem{AOperand{bf(W.h_kv) + kC, 2 * kC, 0, 0}, P + L.w_v2, kC, R, kC, kC, plain_epilogue(bf(W.y_v), kC, wf(L.b_v2), 0)};
-    g[2].ep.stats_out = stats_v;
-    g[3] = GemmItem{AOperand{bf(W.q), kC, 0, 0}, P + L.w_q, kC, Q, kC, kC, plain_epilogue(bf(W.y_q), kC, nullptr, 0)};
-    g[3].ep.stats_out = stats_q;
-    for (int i = 1; i <= 3; ++i) {
-      g[i].ep.stats_out_slots = kStatSlots;
-      g[i].stage = 1;
-    }
+    GemmItem g[8], in_proj[3];
+    stage12_items(g, f, P, L, nullptr, bufs, R, Q);
+    for (int i = 1; i <= 3; ++i) g[i].stage = 1;
     g[1].ep.wm_s = g[2].ep.wm_s = s;
     g[1].dep = g[2].dep = 0;
     g[3].dep = kDepFront;
-    g[4] = GemmItem{AOperand{bf(W.y_q), kC, 0, 0}, P + L.w_iq, kC, Q, kC, kC, plain_epilogue(bf(W.q_p), kC, wf(L.c_q), 0)};
-    g[4].ep.col_a = wf(L.wsum_q);
-    g[4].ep.stats_in = stats_q;
-    g[4].ep.stats_in_slots = kStatSlots;
-    g[4].ep.alpha = 0.08838834764831845f;   // 1/sqrt(head_dim = 128): torch MHA scales q after the in-projection
+    stage3_items(in_proj, P, L, bufs, R, Q);
+    g[4] = in_proj[2];
     g[4].stage = 2;
     g[4].dep = 3;
     g[5] = GemmItem{AOperand{bf(W.y_k), kC, 0, 0}, P + L.w_ik, kC, R, kC, kC, plain_epilogue(nullptr, kC, nullptr, 0)};
@@ -1076,8 +1108,8 @@ int forward_impl(const void* packed, const void* x0, const void* xm, const void*
     g[5].b2 = P + L.w_iv;
     g[5].attn.qp = bf(W.q_p);
     g[5].attn.ctx = bf(W.ctx);
-    g[5].attn.stats_k = stats_k;
-    g[5].attn.stats_v = stats_v;
+    g[5].attn.stats_k = bufs.stats_k;
+    g[5].attn.stats_v = bufs.stats_v;
     g[5].attn.wsum_k = wf(L.wsum_k);
     g[5].attn.cst_k = wf(L.c_k);
     g[5].attn.wsum_v = wf(L.wsum_v);
@@ -1106,11 +1138,11 @@ int forward_impl(const void* packed, const void* x0, const void* xm, const void*
     g[7].dep = 6;
     FwdKey key;
     memset(&key, 0, sizeof(key));
-    key.packed = packed; key.x0 = x0; key.xm = xm; key.out = out; key.ws = workspace;
-    for (int i = 0; i < 4; ++i) key.layers[i] = xm_layers != nullptr ? xm_layers[i] : nullptr;
+    key.packed = packed; key.x0 = f.x0; key.out = out; key.ws = workspace;
+    for (int i = 0; i < 4; ++i) key.xm[i] = f.xm[i];
     for (int i = 0; i < n_peers && i < kMaxPeers; ++i) key.peers[i] = peer_out[i];
-    key.n = n_crops; key.s0 = x0_crop_stride; key.sm = xm_crop_stride; key.crop_rows = out_crop_rows;
-    key.s = s; key.H = H; key.n_peers = n_peers; key.sms = dev.sms;
+    key.n = n_crops; key.s0 = f.x0_crop_stride; key.sm = f.xm_crop_stride; key.crop_rows = out_crop_rows;
+    key.s = s; key.H = H; key.n_peers = n_peers; key.sms = dev.sms; key.parts = f.parts;
     if (chain_feasible(g, 8, dev.sms, false)) {
       for (FwdPlan& fp : g_fwd_plans)
         if (fp.valid && memcmp(&fp.key, &key, sizeof(key)) == 0) {
@@ -1127,52 +1159,20 @@ int forward_impl(const void* packed, const void* x0, const void* xm, const void*
       return TP_OK;
     }
   }
-  // k' / v' have buffers of their own: in a chained launch [3] runs while other row blocks of [2] still read h_kv, so the
-  // round-1 trick of writing them over the dead h_kv buffer is no longer legal
-  __nv_bfloat16* k_p = bf(W.k_p);
-  __nv_bfloat16* v_p = bf(W.v_p);
   {
     GemmItem g[7];
-    AOperand a{xm, xm_width, 0, 0};
-    if (xm_crop_stride != static_cast<int64_t>(kTokens) * xm_width) a = AOperand{xm, xm_width, kTokens, xm_crop_stride};
-    if (xm_layers != nullptr) {
-      a.parts = 4;
-      for (int i = 1; i < 4; ++i) a.more[i - 1] = xm_layers[i];
-    }
-    g[0] = GemmItem{a, P + L.w_kv0, kCm, R, 2 * kC, kCm, plain_epilogue(bf(W.h_kv), 2 * kC, wf(L.b_kv0), 1)};
-    g[0].stage = 0;
-    g[1] = GemmItem{AOperand{bf(W.h_kv), 2 * kC, 0, 0}, P + L.w_k2, kC, R, kC, kC, plain_epilogue(bf(W.y_k), kC, wf(L.b_k2), 0)};
-    g[1].ep.stats_out = stats_k;
-    g[1].ep.stats_out_slots = kStatSlots;
-    g[2] = GemmItem{AOperand{bf(W.h_kv) + kC, 2 * kC, 0, 0}, P + L.w_v2, kC, R, kC, kC, plain_epilogue(bf(W.y_v), kC, wf(L.b_v2), 0)};
-    g[2].ep.stats_out = stats_v;
-    g[2].ep.stats_out_slots = kStatSlots;
-    g[3] = GemmItem{AOperand{bf(W.q), kC, 0, 0}, P + L.w_q, kC, Q, kC, kC, plain_epilogue(bf(W.y_q), kC, nullptr, 0)};
-    g[3].ep.stats_out = stats_q;
-    g[3].ep.stats_out_slots = kStatSlots;
+    stage12_items(g, f, P, L, nullptr, bufs, R, Q);
+    stage3_items(g + 4, P, L, bufs, R, Q);
     g[1].stage = g[2].stage = g[3].stage = 1;
     g[1].dep = g[2].dep = 0;
     g[3].dep = kDepFront;
-    g[4] = GemmItem{AOperand{bf(W.y_k), kC, 0, 0}, P + L.w_ik, kC, R, kC, kC, plain_epilogue(k_p, kC, wf(L.c_k), 0)};
-    g[4].ep.col_a = wf(L.wsum_k);
-    g[4].ep.stats_in = stats_k;
-    g[4].ep.stats_in_slots = kStatSlots;
-    g[5] = GemmItem{AOperand{bf(W.y_v), kC, 0, 0}, P + L.w_iv, kC, R, kC, kC, plain_epilogue(v_p, kC, wf(L.c_v), 0)};
-    g[5].ep.col_a = wf(L.wsum_v);
-    g[5].ep.stats_in = stats_v;
-    g[5].ep.stats_in_slots = kStatSlots;
-    g[6] = GemmItem{AOperand{bf(W.y_q), kC, 0, 0}, P + L.w_iq, kC, Q, kC, kC, plain_epilogue(bf(W.q_p), kC, wf(L.c_q), 0)};
-    g[6].ep.col_a = wf(L.wsum_q);
-    g[6].ep.stats_in = stats_q;
-    g[6].ep.stats_in_slots = kStatSlots;
-    g[6].ep.alpha = 0.08838834764831845f;   // 1/sqrt(head_dim = 128): torch MHA scales q after the in-projection
     g[4].stage = g[5].stage = g[6].stage = 2;
     g[4].dep = 1;
     g[5].dep = 2;
     g[6].dep = 3;
     TP_TRY(launch_chain(g, 7, flags, flags_a + (Q + 255) / 256 + 1, &front, dev.sms, stream));
   }
-  TP_TRY(launch_attn_s(s, bf(W.q_p), k_p, v_p, bf(W.ctx), Q, stream));
+  TP_TRY(launch_attn_s(s, bufs.q_p, bufs.k_p, bufs.v_p, bf(W.ctx), Q, stream));
   {
     GemmItem g[2];
     g[0] = GemmItem{AOperand{bf(W.ctx), kC, 0, 0}, P + L.w_om, kC, Q, H, kC, plain_epilogue(bf(W.h_m), H, wf(L.b_om), 1)};
@@ -1203,21 +1203,25 @@ extern "C" {
 int tp_forward(const void* packed, const void* x0, const void* xm, int64_t n_crops, int64_t x0_crop_stride, int64_t xm_crop_stride,
                int scale_factor, int hidden, void* out, const int64_t* seg_row_offset, void* workspace, size_t workspace_bytes,
                void* stream) {
-  return forward_impl(packed, x0, xm, nullptr, n_crops, x0_crop_stride, xm_crop_stride, scale_factor, hidden, out, seg_row_offset, 0, nullptr, 0,
-                      workspace, workspace_bytes, stream);
+  return forward_impl(packed, Features::cat(x0, x0_crop_stride, xm, xm_crop_stride), n_crops, scale_factor, hidden, out, seg_row_offset, 0,
+                      nullptr, 0, workspace, workspace_bytes, stream);
 }
 
 int tp_forward_packed(const void* packed, const void* x0, const void* xm, int64_t n_crops, int64_t x0_crop_stride, int64_t xm_crop_stride,
                       int scale_factor, int hidden, void* out, int64_t out_crop_rows, void* workspace, size_t workspace_bytes, void* stream) {
-  return forward_impl(packed, x0, xm, nullptr, n_crops, x0_crop_stride, xm_crop_stride, scale_factor, hidden, out, nullptr, out_crop_rows, nullptr,
-                      0, workspace, workspace_bytes, stream);
+  return forward_impl(packed, Features::cat(x0, x0_crop_stride, xm, xm_crop_stride), n_crops, scale_factor, hidden, out, nullptr, out_crop_rows,
+                      nullptr, 0, workspace, workspace_bytes, stream);
 }
 
 int tp_forward_layers(const void* packed, const void* const* layers, int64_t n_crops, int64_t crop_stride, int scale_factor, int hidden,
                       void* out, const int64_t* seg_row_offset, void* workspace, size_t workspace_bytes, void* stream) {
-  if (layers == nullptr) return TP_ERR_INVALID_ARGUMENT;
-  return forward_impl(packed, layers[3], nullptr, layers, n_crops, crop_stride, crop_stride, scale_factor, hidden, out, seg_row_offset, 0,
-                      nullptr, 0, workspace, workspace_bytes, stream);
+  // (a missing layer is reported before a bad scale factor)
+  if (layers == nullptr || layers[0] == nullptr || layers[1] == nullptr || layers[2] == nullptr || layers[3] == nullptr)
+    return TP_ERR_INVALID_ARGUMENT;
+  if (scale_factor <= 0 || kGrid % scale_factor != 0) return TP_ERR_BAD_SCALE_FACTOR;
+  TP_TRY(check_layers(layers, crop_stride));
+  return forward_impl(packed, Features::layers(layers, crop_stride), n_crops, scale_factor, hidden, out, seg_row_offset, 0, nullptr, 0,
+                      workspace, workspace_bytes, stream);
 }
 
 int tp_forward_layers_packed(const void* packed, const void* const* layers, int64_t n_crops, int64_t crop_stride, int scale_factor,
@@ -1228,8 +1232,8 @@ int tp_forward_layers_packed(const void* packed, const void* const* layers, int6
   if ((reinterpret_cast<uintptr_t>(out) & 15) != 0 || !valid_hidden(hidden) ||
       (out_crop_rows != 0 && (out_crop_rows < mq || out_crop_rows > 0x7fffffffll / hidden)))
     return TP_ERR_INVALID_ARGUMENT;
-  return forward_impl(packed, layers[3], nullptr, layers, n_crops, crop_stride, crop_stride, scale_factor, hidden, out, nullptr, out_crop_rows,
-                      nullptr, 0, workspace, workspace_bytes, stream);
+  return forward_impl(packed, Features::layers(layers, crop_stride), n_crops, scale_factor, hidden, out, nullptr, out_crop_rows, nullptr, 0,
+                      workspace, workspace_bytes, stream);
 }
 
 int tp_forward_allgather(const void* packed, const void* x0, const void* xm, int64_t n_crops, int64_t x0_crop_stride,
@@ -1249,8 +1253,8 @@ int tp_forward_allgather(const void* packed, const void* x0, const void* xm, int
     if (peer_out[p] == nullptr) return TP_ERR_INVALID_ARGUMENT;
     dst[p] = static_cast<uint8_t*>(peer_out[p]) + slot;
   }
-  return forward_impl(packed, x0, xm, nullptr, n_crops, x0_crop_stride, xm_crop_stride, scale_factor, hidden, dst[0], nullptr, out_crop_rows, dst,
-                      n_peers, workspace, workspace_bytes, stream);
+  return forward_impl(packed, Features::cat(x0, x0_crop_stride, xm, xm_crop_stride), n_crops, scale_factor, hidden, dst[0], nullptr,
+                      out_crop_rows, dst, n_peers, workspace, workspace_bytes, stream);
 }
 
 namespace {

@@ -228,12 +228,7 @@ __global__ void __launch_bounds__(256) window_attn_stream_kernel(const __nv_bflo
 // ------------------------------------------------------------------------------------------------
 // Weight packing
 // ------------------------------------------------------------------------------------------------
-__global__ void bf16_to_f32_kernel(const __nv_bfloat16* __restrict__ src, float* __restrict__ dst, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) dst[i] = __bfloat162float(src[i]);
-}
-
-// Several bf16 -> fp32 vectors in one launch (the biases of a training-step repack): blockIdx.y = segment
+// bf16 -> fp32 vectors in one launch (the packed biases): blockIdx.y = segment
 struct CastSeg { const __nv_bfloat16* src; float* dst; int n; };
 struct CastSegs { CastSeg s[8]; };
 __global__ void bf16_to_f32_multi_kernel(CastSegs segs) {
@@ -268,15 +263,6 @@ __global__ void fold_layernorm_kernel(const __nv_bfloat16* __restrict__ w, const
     wsum[o] = s;
     cst[o] = c + __bfloat162float(bias[o]);
   }
-}
-
-// out[c, r] = in[r, c] for a square bf16 matrix (pack time only: W_o^T as the K-major B operand of the fold GEMM)
-__global__ void transpose_bf16_kernel(const __nv_bfloat16* __restrict__ in, __nv_bfloat16* __restrict__ out, int n) {
-  __shared__ __nv_bfloat16 tile[32][33];
-  const int bx = blockIdx.x * 32, by = blockIdx.y * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) tile[i][threadIdx.x] = in[static_cast<long long>(by + i) * n + bx + threadIdx.x];
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) out[static_cast<long long>(bx + i) * n + by + threadIdx.x] = tile[threadIdx.x][i];
 }
 
 // out[o] = sum_i w[o, i] * x[i] + b[o]   (fp32 out; one warp per output; pack time only)
