@@ -1,9 +1,10 @@
-// Test-only entry points into the backward's internal kernels and the forward's buffer layouts (libtokenpacker_b200_testhooks.so,
-// loaded by tests/test_train_kernels_gpu.py, tests/test_forward_stages_gpu.py and tests/test_train_stages_gpu.py; never by the
-// package).  The library is the product translation unit plus the tpt_* functions
-// below, which call the same launch functions tp_backward calls (tp_train.inl), so every kernel runs with the launch configuration
-// of a training step.  Conventions as in include/tokenpacker_b200.h: device pointers, caller-owned buffers, work enqueued on
-// ``stream``, a tp_status returned.
+// Test-only entry points into the backward's internal kernels, the forward's buffer layouts and the GEMM engine
+// (libtokenpacker_b200_testhooks.so, loaded by tests/test_train_kernels_gpu.py, tests/test_forward_stages_gpu.py,
+// tests/test_train_stages_gpu.py and tests/test_gemm_engine_gpu.py; never by the package).  The library is the product translation
+// unit plus the tpt_* functions below, which call the same launch functions tp_backward calls (tp_train.inl), so every kernel runs
+// with the launch configuration of a training step; the tpt_gemm_* functions hand arbitrary items straight to launch_gemms /
+// launch_chain with a caller-chosen SM count.  Conventions as in include/tokenpacker_b200.h: device pointers, caller-owned buffers,
+// work enqueued on ``stream``, a tp_status returned.
 #include "../../tokenpacker_b200/csrc/tp_api.cu"
 
 extern "C" {
@@ -156,6 +157,113 @@ TP_API int tpt_packed_layout(int hidden, int64_t* out) {
 TP_API int tpt_transpose(const void* in, int64_t ld_in, void* out, int64_t ld_out, int64_t rows, int cols, void* stream) {
   if (in == nullptr || out == nullptr || rows <= 0 || cols <= 0 || ld_in < cols || ld_out < rows) return TP_ERR_INVALID_ARGUMENT;
   return launch_transpose(in, ld_in, out, ld_out, rows, cols, static_cast<cudaStream_t>(stream));
+}
+
+// ---- the GEMM engine on its own (tests/test_gemm_engine_gpu.py) ----
+// One non-attention GemmItem as a flat C struct (mirrored field by field in Python; tpt_gemm_desc_size guards the layout).  Every
+// field maps onto the GemmItem / GemmEpilogue member of the same meaning; the LayerNorm epsilon is the product's 1e-6.
+struct tpt_gemm_desc {
+  int32_t tn;                        // 0: C = A . B^T;  1: C = A^T . B (A [K, M], B [K, N] row-major);  2: C = A . B (B [K, N] row-major)
+  int32_t a_parts;                   // A as a_parts tensors side by side along K (a, a_more[0..]); 0 means 1
+  const void* a;
+  const void* a_more[3];
+  int64_t lda, a_seg_rows, a_seg_stride;
+  const void* b;
+  const void* b_more[3];
+  int64_t ldb;
+  int32_t b_parts;                   // TN only: B as b_parts tensors side by side along N; 0 means 1
+  int32_t pad0;
+  int64_t b_seg_rows, b_seg_stride;
+  int64_t M, N, K;
+  void* c;
+  int64_t ldc;
+  const float* bias;                 // col_b
+  const float* col_a;                // LayerNorm fold (with stats_in, stats_in_slots, ln_inv_dim)
+  const float* stats_in;
+  float* stats_out;
+  const int64_t* seg_row_offset;
+  int32_t stats_in_slots, stats_out_slots;
+  float ln_inv_dim, alpha;
+  int32_t gelu, dual;
+  void* c_pre;
+  int64_t ld_pre;
+  int32_t out_f32, k_splits;
+  int32_t seg_len, seg_stride;
+  int32_t stage, dep;                // tpt_gemm_chain only
+};
+
+TP_API int tpt_gemm_desc_size(void) { return static_cast<int>(sizeof(tpt_gemm_desc)); }
+
+static GemmItem gemm_item_of(const tpt_gemm_desc& d) {
+  GemmItem it{};
+  it.a.ptr = d.a;
+  it.a.ld = d.lda;
+  it.a.seg_rows = d.a_seg_rows;
+  it.a.seg_stride = d.a_seg_stride;
+  it.a.parts = d.a_parts > 0 ? d.a_parts : 1;
+  for (int i = 0; i < 3; ++i) {
+    it.a.more[i] = d.a_more[i];
+    it.b_more[i] = d.b_more[i];
+  }
+  it.b = d.b;
+  it.ldb = d.ldb;
+  it.b_parts = d.b_parts > 0 ? d.b_parts : 1;
+  it.b_seg_rows = d.b_seg_rows;
+  it.b_seg_stride = d.b_seg_stride;
+  it.M = d.M;
+  it.N = d.N;
+  it.K = d.K;
+  it.tn = d.tn;
+  it.ep = plain_epilogue(d.c, d.ldc, d.bias, d.gelu);
+  it.ep.alpha = d.alpha;
+  it.ep.col_a = d.col_a;
+  it.ep.stats_in = d.stats_in;
+  it.ep.stats_in_slots = d.stats_in_slots;
+  it.ep.ln_inv_dim = d.ln_inv_dim;
+  it.ep.stats_out = d.stats_out;
+  it.ep.stats_out_slots = d.stats_out_slots;
+  it.ep.seg_row_offset = reinterpret_cast<const long long*>(d.seg_row_offset);
+  it.ep.seg_len = d.seg_len;
+  it.ep.seg_stride = d.seg_stride;
+  it.ep.dual = d.dual;
+  it.ep.out_f32 = d.out_f32;
+  it.c_pre = d.c_pre;
+  it.ld_pre = d.ld_pre;
+  it.k_splits = d.k_splits;
+  it.stage = d.stage;
+  it.dep = d.dep;
+  return it;
+}
+
+// Up to one item more than a launch takes, so that the engine's own count check is what refuses it.
+constexpr int kMaxDescs = kMaxGroup + 1;
+
+static int gemm_items_of(const tpt_gemm_desc* items, int count, GemmItem* out) {
+  if (items == nullptr || count <= 0 || count > kMaxDescs) return TP_ERR_INVALID_ARGUMENT;
+  for (int i = 0; i < count; ++i) out[i] = gemm_item_of(items[i]);
+  return TP_OK;
+}
+
+// The items in ONE call of launch_gemms with the caller's SM count (grid sizes and, through them, every CTA's tile sequence).
+TP_API int tpt_gemm_group(const tpt_gemm_desc* items, int count, int sms, void* stream) {
+  GemmItem it[kMaxDescs];
+  TP_TRY(gemm_items_of(items, count, it));
+  return launch_gemms(it, count, sms, static_cast<cudaStream_t>(stream));
+}
+
+// The items as one launch_chain (sorted by stage; dep = index of the producer of an item's A, or -1) with the caller's SM count;
+// flags: caller-zeroed int32 tile counters, flag_capacity of them.  Plain GEMM -> GEMM chains only (no front work).
+TP_API int tpt_gemm_chain(const tpt_gemm_desc* items, int count, int* flags, int64_t flag_capacity, int sms, void* stream) {
+  GemmItem it[kMaxDescs];
+  TP_TRY(gemm_items_of(items, count, it));
+  return launch_chain(it, count, flags, flag_capacity, nullptr, sms, static_cast<cudaStream_t>(stream));
+}
+
+// choose_kernel's answer for this item in a launch of `count` items under the current TP_GEMM_MODE: 0 pair kernel, 1 one-CTA
+// 128 x 256, 2 one-CTA 128 x 128, -1 none can run it.
+TP_API int tpt_gemm_choice(const tpt_gemm_desc* item, int count, int sms) {
+  if (item == nullptr) return -1;
+  return choose_kernel(gemm_item_of(*item), count, sms, gemm_mode());
 }
 
 }  // extern "C"

@@ -226,12 +226,15 @@ int make_a_map(CUtensorMap* map, const AOperand& a, long long M, long long K) {
   return make_map_3d(map, a.ptr, M / a.seg_rows, a.seg_rows, K, a.ld, a.seg_stride);
 }
 
+// Operand maps of a one-CTA launch with 128 x block_n tiles (encoded before anything of the call is launched).
+int make_one_cta_maps(const GemmItem& it, int block_n, CUtensorMap* map_a, CUtensorMap* map_b) {
+  TP_TRY(make_a_map(map_a, it.a, it.M, it.K));
+  return make_map_2d(map_b, it.b, it.N, it.K, it.ldb, block_n);
+}
+
 template <int kBlockN>
-int launch_gemm_t(const GemmItem& it, int sms, cudaStream_t stream) {
+int launch_gemm_t(const GemmItem& it, const CUtensorMap& map_a, const CUtensorMap& map_b, int sms, cudaStream_t stream) {
   using Cfg = GemmConfig<kBlockN>;
-  CUtensorMap map_a, map_b;
-  TP_TRY(make_a_map(&map_a, it.a, it.M, it.K));
-  TP_TRY(make_map_2d(&map_b, it.b, it.N, it.K, it.ldb, kBlockN));
   {
     static thread_local unsigned attr_done = 0;        // bit per device: the attribute is per (function, device)
     int dev = 0;
@@ -257,11 +260,10 @@ struct BuiltLaunch {
   int grid;
 };
 
-// Up to kMaxGroup independent problems in ONE launch of the CTA-pair kernel.
-int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream_t stream, const FrontWork* front = nullptr,
-                           BuiltLaunch* built = nullptr) {
+// Up to kMaxGroup independent problems for ONE launch of the CTA-pair kernel: every check, tensor map and the grid, nothing launched.
+int build_pair_group(const GemmItem* items, int count, int sms, const FrontWork* front, BuiltLaunch* out) {
   using Cfg = Gemm2Config;
-  GemmGroup g;
+  GemmGroup& g = out->g;
   memset(&g, 0, sizeof(g));
   g.count = count;
   long long total = 0;
@@ -396,7 +398,7 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
   if (total > 0x7fffffffll) return TP_ERR_INVALID_ARGUMENT;
   g.total_tiles = static_cast<int>(total);
   if (front != nullptr) g.front = *front;
-  PeerStores peers;
+  PeerStores& peers = out->peers;
   memset(&peers, 0, sizeof(peers));
   int peer_item = -1;
   // The destination maps of the launch: the peers of a fused all-gather, or — for a segmented (packed-row) output that stays on this
@@ -466,6 +468,16 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
     peers.whole = whole ? 1 : 0;
     g.p[peer_item].peer_out = 1;
   }
+  const long long max_pairs = sms / 2;
+  const int grid = 2 * static_cast<int>(total < max_pairs ? total : max_pairs);
+  for (int i = 0; i < count; ++i)
+    if (g.p[i].dep_shift == 31) g.p[i].dep_target = grid;        // front work: one arrival per CTA of this launch
+  out->grid = grid;
+  return TP_OK;
+}
+
+int launch_built(const BuiltLaunch& b, cudaStream_t stream) {
+  using Cfg = Gemm2Config;
   {
     static thread_local unsigned attr_done = 0;
     int dev = 0;
@@ -475,17 +487,17 @@ int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream
       if (dev < 32) attr_done |= 1u << dev;
     }
   }
-  const long long max_pairs = sms / 2;
-  const int grid = 2 * static_cast<int>(total < max_pairs ? total : max_pairs);
-  for (int i = 0; i < count; ++i)
-    if (g.p[i].dep_shift == 31) g.p[i].dep_target = grid;        // front work: one arrival per CTA of this launch
-  TP_CUDA(launch_pdl(tp_gemm2_kernel, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, g, peers));
-  if (built != nullptr) {
-    built->g = g;
-    built->peers = peers;
-    built->grid = grid;
-  }
+  TP_CUDA(launch_pdl(tp_gemm2_kernel, dim3(b.grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, b.g, b.peers));
   return TP_OK;
+}
+
+// Build and launch; built != nullptr: the launch is kept there for replay (the forward plan cache)
+int launch_gemm_pair_group(const GemmItem* items, int count, int sms, cudaStream_t stream, const FrontWork* front = nullptr,
+                           BuiltLaunch* built = nullptr) {
+  BuiltLaunch local;
+  BuiltLaunch* b = built != nullptr ? built : &local;
+  TP_TRY(build_pair_group(items, count, sms, front, b));
+  return launch_built(*b, stream);
 }
 
 // Kernel selection: CTA-pair 256x256 tiles whenever the problem fills them (independent problems of one stage share a
@@ -539,24 +551,36 @@ int gemm_mode() {
 int launch_gemms(const GemmItem* items, int count, int sms, cudaStream_t stream) {
   if (count <= 0 || count > kMaxGroup) return TP_ERR_INVALID_ARGUMENT;
   const int mode = gemm_mode();
+  // Every item is checked, placed and encoded before the first launch: an invalid item anywhere in the list launches nothing.
+  int choice[kMaxGroup];
+  CUtensorMap map_a[kMaxGroup], map_b[kMaxGroup];     // one-CTA items
   GemmItem grouped[kMaxGroup];
   int n_grouped = 0;
+  BuiltLaunch pair;
   for (int i = 0; i < count; ++i) {
     TP_TRY(check_item(items[i]));
     const GemmItem& it = items[i];
     if (it.n_peers > 0 && count != 1) return TP_ERR_INVALID_ARGUMENT;
-    const int choice = choose_kernel(it, count, sms, mode);
-    if (choice < 0) return TP_ERR_INVALID_ARGUMENT;
-    if (choice == 0) {
-      if (mode == 3) TP_TRY(launch_gemm_pair_group(&it, 1, sms, stream));
+    choice[i] = choose_kernel(it, count, sms, mode);
+    if (choice[i] < 0) return TP_ERR_INVALID_ARGUMENT;
+    if (choice[i] == 0) {
+      if (mode == 3) TP_TRY(build_pair_group(&it, 1, sms, nullptr, &pair));     // validated here, rebuilt at its launch below
       else grouped[n_grouped++] = it;
-    } else if (choice == 1) {
-      TP_TRY(launch_gemm_t<256>(it, sms, stream));
     } else {
-      TP_TRY(launch_gemm_t<128>(it, sms, stream));
+      TP_TRY(make_one_cta_maps(it, choice[i] == 1 ? 256 : 128, &map_a[i], &map_b[i]));
     }
   }
-  if (n_grouped > 0) TP_TRY(launch_gemm_pair_group(grouped, n_grouped, sms, stream));
+  if (n_grouped > 0) TP_TRY(build_pair_group(grouped, n_grouped, sms, nullptr, &pair));
+  for (int i = 0; i < count; ++i) {
+    if (choice[i] == 0) {
+      if (mode == 3) TP_TRY(launch_gemm_pair_group(&items[i], 1, sms, stream));
+    } else if (choice[i] == 1) {
+      TP_TRY(launch_gemm_t<256>(items[i], map_a[i], map_b[i], sms, stream));
+    } else {
+      TP_TRY(launch_gemm_t<128>(items[i], map_a[i], map_b[i], sms, stream));
+    }
+  }
+  if (n_grouped > 0) TP_TRY(launch_built(pair, stream));
   return TP_OK;
 }
 
