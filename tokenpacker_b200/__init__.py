@@ -10,6 +10,7 @@ from .projector import TokenPackerB200, TokenPacker, build_vision_projector, Ide
 from .hd import Image_Patch, hd_grid, hd_tile, hd_tile_batch, hd_preprocess_batch, hd_plan, hd_assemble, hd_seq_len
 from .clip import clip_preprocess_batch
 from .splice import splice_multimodal, splice_plan
+from .tower import CLIPVisionTowerB200
 
 __all__ = ["TokenPackerB200", "TokenPacker", "build_vision_projector", "IdentityMap", "Image_Patch", "hd_grid", "hd_tile", "hd_tile_batch",
-           "hd_preprocess_batch", "hd_plan", "hd_assemble", "hd_seq_len", "clip_preprocess_batch", "splice_multimodal", "splice_plan"]
+           "hd_preprocess_batch", "hd_plan", "hd_assemble", "hd_seq_len", "clip_preprocess_batch", "splice_multimodal", "splice_plan", "CLIPVisionTowerB200"]

@@ -2,7 +2,7 @@
 
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
 Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
-include/tokenpacker_b200_input_grad.h and include/tokenpacker_b200_layers.h one to one.
+include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h and include/tokenpacker_b200_clip_tower.h one to one.
 """
 from __future__ import annotations
 
@@ -145,6 +145,41 @@ LAYERS_SIGNATURES = {
                                            C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
+# the same for include/tokenpacker_b200_clip_tower.h (the frozen CLIP vision tower, forward only)
+CLIP_TOWER_LAYERS = 23
+CLIP_TOWER_LAYER_FIELDS = [
+    # (struct field, parameter name inside encoder.layers.{i})
+    ("ln1_w", "layer_norm1.weight"), ("ln1_b", "layer_norm1.bias"),
+    ("q_w", "self_attn.q_proj.weight"), ("q_b", "self_attn.q_proj.bias"),
+    ("k_w", "self_attn.k_proj.weight"), ("k_b", "self_attn.k_proj.bias"),
+    ("v_w", "self_attn.v_proj.weight"), ("v_b", "self_attn.v_proj.bias"),
+    ("o_w", "self_attn.out_proj.weight"), ("o_b", "self_attn.out_proj.bias"),
+    ("ln2_w", "layer_norm2.weight"), ("ln2_b", "layer_norm2.bias"),
+    ("fc1_w", "mlp.fc1.weight"), ("fc1_b", "mlp.fc1.bias"),
+    ("fc2_w", "mlp.fc2.weight"), ("fc2_b", "mlp.fc2.bias"),
+]
+CLIP_TOWER_FIELDS = [
+    ("patch_w", "embeddings.patch_embedding.weight"), ("class_emb", "embeddings.class_embedding"),
+    ("pos_emb", "embeddings.position_embedding.weight"), ("pre_ln_w", "pre_layrnorm.weight"), ("pre_ln_b", "pre_layrnorm.bias"),
+]
+
+
+class TpClipTowerLayer(C.Structure):
+    _fields_ = [(name, C.c_void_p) for name, _ in CLIP_TOWER_LAYER_FIELDS]
+
+
+class TpClipTowerWeights(C.Structure):
+    _fields_ = [(name, C.c_void_p) for name, _ in CLIP_TOWER_FIELDS] + [("layers", TpClipTowerLayer * CLIP_TOWER_LAYERS)]
+
+
+CLIP_TOWER_SIGNATURES = {
+    "tp_clip_tower_packed_bytes": (C.c_size_t, []),
+    "tp_clip_tower_pack_weights": (C.c_int, [C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "tp_clip_tower_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "tp_clip_tower_forward": (C.c_int, [C.c_void_p, C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_int64, C.c_int64, C.POINTER(C.c_void_p),
+                                        C.c_void_p, C.c_size_t, C.c_void_p]),
+}
+
 
 def _load():
     if not os.path.exists(LIB_PATH):
@@ -153,7 +188,7 @@ def _load():
             "(or `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
-                                      **LAYERS_SIGNATURES}.items():
+                                      **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/tokenpacker_b200.h"
+#include "../../include/tokenpacker_b200_clip_tower.h"
 #include "../../include/tokenpacker_b200_clip_u8.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"
@@ -19,6 +20,7 @@
 #include "tp_gemm.cuh"
 #include "tp_kernels.cuh"
 #include "tp_backward.cuh"
+#include "tp_clip_tower.cuh"
 
 namespace {
 
@@ -208,6 +210,8 @@ struct GemmItem {
 };
 constexpr int kDepFront = -2;      // GemmItem::dep: the A operand is the point-query output of the launch's front work
 
+bool tower_epilogue(const GemmEpilogue& ep);
+
 int check_item(const GemmItem& it) {
   if (it.kind == 1) return (it.M > 0 && it.M % 16 == 0 && it.attn.qp != nullptr && it.attn.ctx != nullptr) ? TP_OK : TP_ERR_INVALID_ARGUMENT;
   if (it.M <= 0 || it.N <= 0 || it.K <= 0 || it.N % 32 != 0 || it.M > 0x7fffff00ll) return TP_ERR_INVALID_ARGUMENT;   // K: any (TMA zero-fills)
@@ -217,6 +221,14 @@ int check_item(const GemmItem& it) {
   if (it.ep.stats_out != nullptr && (it.N % 256 != 0 || it.ep.stats_out_slots != it.N / 128)) return TP_ERR_INVALID_ARGUMENT;
   if (it.ep.col_a != nullptr && (it.ep.stats_in == nullptr || it.ep.stats_in_slots <= 0)) return TP_ERR_INVALID_ARGUMENT;
   if ((it.b_parts != 1 || it.b_seg_rows != 0) && it.tn != 1) return TP_ERR_INVALID_ARGUMENT;
+  // the tower's epilogue instantiations (tower_epilogue) have no erf GELU, LayerNorm fold, row statistics, dual, window-major or fp32
+  // output, no KV-attention tiles and no TN / NN operand forms; R is read 16 bytes at a time
+  if (tower_epilogue(it.ep) && (it.ep.gelu == 1 || it.ep.col_a != nullptr || it.ep.stats_out != nullptr || it.ep.dual || it.ep.wm_s != 0 ||
+                                it.k_splits != 1 || it.kind != 0 || it.tn != 0 ||
+                                (reinterpret_cast<uintptr_t>(it.ep.resid) & 15) != 0 || it.ep.ldr % 8 != 0))
+    return TP_ERR_INVALID_ARGUMENT;
+  if (it.ep.resid_f32 && it.ep.resid == nullptr) return TP_ERR_INVALID_ARGUMENT;
+  if (it.ep.gelu < 0 || it.ep.gelu > 2) return TP_ERR_INVALID_ARGUMENT;
   return TP_OK;
 }
 
@@ -232,24 +244,33 @@ int make_one_cta_maps(const GemmItem& it, int block_n, CUtensorMap* map_a, CUten
   return make_map_2d(map_b, it.b, it.N, it.K, it.ldb, block_n);
 }
 
-template <int kBlockN>
-int launch_gemm_t(const GemmItem& it, const CUtensorMap& map_a, const CUtensorMap& map_b, int sms, cudaStream_t stream) {
+// The CLIP tower's epilogue features (residual add, quick_gelu) run in instantiations of their own (tp_gemm.cuh: kTower)
+bool tower_epilogue(const GemmEpilogue& ep) { return ep.resid != nullptr || ep.gelu == 2; }   // (an fp32 output alone stays on the projector's)
+
+template <int kBlockN, bool kTower>
+int launch_gemm_tt(const GemmItem& it, const CUtensorMap& map_a, const CUtensorMap& map_b, int sms, cudaStream_t stream) {
   using Cfg = GemmConfig<kBlockN>;
   {
     static thread_local unsigned attr_done = 0;        // bit per device: the attribute is per (function, device)
     int dev = 0;
     TP_CUDA(cudaGetDevice(&dev));
     if (dev >= 32 || !(attr_done & (1u << dev))) {
-      TP_CUDA(cudaFuncSetAttribute(tp_gemm_kernel<kBlockN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+      TP_CUDA(cudaFuncSetAttribute(tp_gemm_kernel<kBlockN, kTower>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
       if (dev < 32) attr_done |= 1u << dev;
     }
   }
   const long long tiles = ((it.M + kBlockM - 1) / kBlockM) * ((it.N + kBlockN - 1) / kBlockN);
   const int grid = static_cast<int>(tiles < sms ? tiles : sms);
   GemmEpilogue ep = it.ep;
-  TP_CUDA(launch_pdl(tp_gemm_kernel<kBlockN>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, map_a, map_b, static_cast<int>(it.M),
-                     static_cast<int>(it.N), static_cast<int>(it.K), static_cast<int>(it.a.seg_rows), ep));
+  TP_CUDA(launch_pdl(tp_gemm_kernel<kBlockN, kTower>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, map_a, map_b,
+                     static_cast<int>(it.M), static_cast<int>(it.N), static_cast<int>(it.K), static_cast<int>(it.a.seg_rows), ep));
   return TP_OK;
+}
+
+template <int kBlockN>
+int launch_gemm_t(const GemmItem& it, const CUtensorMap& map_a, const CUtensorMap& map_b, int sms, cudaStream_t stream) {
+  return tower_epilogue(it.ep) ? launch_gemm_tt<kBlockN, true>(it, map_a, map_b, sms, stream)
+                               : launch_gemm_tt<kBlockN, false>(it, map_a, map_b, sms, stream);
 }
 
 // Everything a launch of the pair kernel needs, as built from a list of items: kept by the forward plan cache below (encoding
@@ -266,6 +287,10 @@ int build_pair_group(const GemmItem* items, int count, int sms, const FrontWork*
   GemmGroup& g = out->g;
   memset(&g, 0, sizeof(g));
   g.count = count;
+  // one launch runs one instantiation (launch_built): tower epilogues and the projector's features never share a group
+  for (int i = 1; i < count; ++i)
+    if (tower_epilogue(items[i].ep) != tower_epilogue(items[0].ep)) return TP_ERR_INVALID_ARGUMENT;
+  if (count > 0 && tower_epilogue(items[0].ep) && front != nullptr) return TP_ERR_INVALID_ARGUMENT;   // no front work there either
   long long total = 0;
   for (int i = 0; i < count; ++i) {
     const GemmItem& it = items[i];
@@ -476,19 +501,26 @@ int build_pair_group(const GemmItem* items, int count, int sms, const FrontWork*
   return TP_OK;
 }
 
-int launch_built(const BuiltLaunch& b, cudaStream_t stream) {
+template <bool kTower>
+int launch_built_t(const BuiltLaunch& b, cudaStream_t stream) {
   using Cfg = Gemm2Config;
   {
     static thread_local unsigned attr_done = 0;
     int dev = 0;
     TP_CUDA(cudaGetDevice(&dev));
     if (dev >= 32 || !(attr_done & (1u << dev))) {
-      TP_CUDA(cudaFuncSetAttribute(tp_gemm2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+      TP_CUDA(cudaFuncSetAttribute(tp_gemm2_kernel<kTower>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
       if (dev < 32) attr_done |= 1u << dev;
     }
   }
-  TP_CUDA(launch_pdl(tp_gemm2_kernel, dim3(b.grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, b.g, b.peers));
+  TP_CUDA(launch_pdl(tp_gemm2_kernel<kTower>, dim3(b.grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, b.g, b.peers));
   return TP_OK;
+}
+
+int launch_built(const BuiltLaunch& b, cudaStream_t stream) {
+  bool tower = false;
+  for (int i = 0; i < b.g.count; ++i) tower = tower || tower_epilogue(b.g.p[i].ep);
+  return tower ? launch_built_t<true>(b, stream) : launch_built_t<false>(b, stream);
 }
 
 // Build and launch; built != nullptr: the launch is kept there for replay (the forward plan cache)
@@ -1171,7 +1203,7 @@ int forward_impl(const void* packed, const Features& f, int64_t n_crops, int sca
       for (FwdPlan& fp : g_fwd_plans)
         if (fp.valid && memcmp(&fp.key, &key, sizeof(key)) == 0) {
           // (the counters were already reset by the memset above)
-          TP_CUDA(launch_pdl(tp_gemm2_kernel, dim3(fp.launch.grid), dim3(kGemmThreads), Gemm2Config::kSmemBytes, stream, fp.launch.g, fp.launch.peers));
+          TP_CUDA(launch_pdl(tp_gemm2_kernel<false>, dim3(fp.launch.grid), dim3(kGemmThreads), Gemm2Config::kSmemBytes, stream, fp.launch.g, fp.launch.peers));
           return TP_OK;
         }
       FwdPlan& slot = g_fwd_plans[g_fwd_next];
@@ -1409,7 +1441,7 @@ int tp_gemm_bf16(const void* a, int64_t lda, const void* b, int64_t ldb, void* c
   if (a == nullptr || b == nullptr || c == nullptr) return TP_ERR_INVALID_ARGUMENT;
   DeviceInfo dev;
   TP_TRY(device_info(&dev));
-  GemmEpilogue ep = plain_epilogue(c, ldc, bias, gelu);
+  GemmEpilogue ep = plain_epilogue(c, ldc, bias, gelu != 0 ? 1 : 0);     // any nonzero flag is the erf GELU, as documented
   ep.alpha = alpha;
   return launch_gemm(AOperand{a, lda, 0, 0}, b, ldb, m, n, k, ep, dev.sms, static_cast<cudaStream_t>(stream));
 }
@@ -1848,3 +1880,5 @@ int tp_hd_fill_separators(void* out, int hidden, const int64_t* sep_rows, int64_
 }
 
 }  // extern "C"
+
+#include "tp_clip_tower.inl"

@@ -30,7 +30,8 @@
 //   v = fma(rstd_r, fma(-mu_r, col_a[c], v), col_b[c])    LayerNorm folded into the NEXT linear: (mu, rstd) from per-row sums,
 //                                                col_b = the folded constant W.beta + b    -- or, without a fold --
 //   v = v + col_b[c]                             bias
-//   v = gelu_erf(v)                              exact erf GELU (nn.GELU default)
+//   v = v + R[r, c]                              residual add (bf16 operand read from global memory)
+//   v = gelu_erf(v)  |  v = quick_gelu(v)        exact erf GELU (nn.GELU default) | x sigmoid(1.702 x) (CLIP)
 //   v = alpha * v                                1/sqrt(head_dim) query scaling
 //   y = bf16(v);  stats_out[r][slot] = (mean, M2) of y over this warp's 128 columns  -> next LayerNorm fold (deterministic:
 //                                                one slot per 128-column block, combined Chan-style in fixed order by the consumer)
@@ -67,6 +68,9 @@ struct GemmEpilogue {
   int dual;                // 1 (with gelu): the bf16-rounded PRE-activation (after bias / LN fold, before GELU and alpha) is stored too,
                            // through GemmProblem::tmap_cx[0] (the training forward keeps z for GELU'(z); builder.py:66-75 under autograd).
                            // Pair kernel, plain (unsegmented) TMA-store output, two 64-column staging buffers per half.
+  const __nv_bfloat16* resid;   // != nullptr: v += resid[row * ldr + c] after bias / LN fold (the CLIP tower's residual stream), read
+  long long ldr;                // straight from global memory (the pair kernel's shared memory is full); row = the GEMM row
+  int resid_f32;                // 1: resid points to float values (the tower's unrounded mid-layer residual x')
 };
 
 constexpr int kBlockM = 128;
@@ -240,13 +244,15 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
   rstd = rsqrtf(__fadd_rn(var, eps));
 }
 
-template <int kTileN>
+// kTower: the CLIP tower's instantiations (bias, bf16 or fp32 residual add, quick_gelu, alpha, fp32 output) — and none of the
+// projector's LayerNorm fold, row statistics, dual / window-major outputs, so that neither set of instantiations carries the other's registers.
+template <int kTileN, bool kTower = false>
 __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int N, const float (&acc)[2][kTileN / 4], uint32_t scratch,
                                               int row, int col_tile0, int quarter, int half, const float* s_col, const OutStage& out,
                                               long long c_extra = 0) {
   constexpr int kColsPerWarp = kTileN / 2;
   constexpr int kChunks = kColsPerWarp / 32;
-  const bool ln_fold = ep.col_a != nullptr;
+  const bool ln_fold = !kTower && ep.col_a != nullptr;
   const bool row_ok = row < M;
   float mu = 0.f, rstd = 1.f;
   // Row statistics arrive as one (mean_i, M2_i) pair per 128-column block (M2 = sum of squared deviations from the block's own
@@ -268,7 +274,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
   const uint32_t out_addr = out.buf != nullptr ? smem_u32(out.buf) : 0u;
 
   float s1 = 0.f, s2 = 0.f, shift = 0.f;     // statistics of (y - shift), shift = the block's first value: sums stay small
-  const bool do_stats = ep.stats_out != nullptr;
+  const bool do_stats = !kTower && ep.stats_out != nullptr;
   const bool scale = ep.alpha != 1.0f;
   const uint64_t rstd2 = pk2(rstd), nmu2 = pk2(-mu), alpha2 = pk2(ep.alpha);
   uint32_t r[32];
@@ -277,7 +283,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
     acc_chunk(acc, chunk, scratch, r);
     const int col0 = col_tile0 + half * kColsPerWarp + chunk * 32;
     // dual output: every 64-column slab exists twice — pre-activation (even slab number, buffer 0) and activation (odd, buffer 1)
-    const bool dual = ep.dual != 0 && out.buf != nullptr;
+    const bool dual = !kTower && ep.dual != 0 && out.buf != nullptr;
     const uint32_t slab_pre = out.slab_seq + 2u * static_cast<uint32_t>(chunk / kChunksPerSlab);
     const uint32_t slab_q = dual ? slab_pre + 1u : out.slab_seq + static_cast<uint32_t>(chunk / kChunksPerSlab);
     const uint32_t slab_buf = slab_q & 1u;
@@ -331,7 +337,32 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
             sts_u4(row_pre + static_cast<uint32_t>((ci ^ swz_pre) << 4), w[0], w[1], w[2], w[3]);
           }
         }
-        if (ep.gelu) {
+        if constexpr (kTower) {
+          if (ep.resid != nullptr && row_ok && ep.resid_f32) {
+            const float4* rp = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(ep.resid) + static_cast<long long>(row) * ep.ldr +
+                                                               col0 + sub * kSubPairs * 2);
+#pragma unroll
+            for (int g = 0; g < kSubPairs / 2; ++g) {
+              const float4 r4 = rp[g];
+              v[2 * g] = add2(v[2 * g], pk2(r4.x, r4.y));
+              v[2 * g + 1] = add2(v[2 * g + 1], pk2(r4.z, r4.w));
+            }
+          } else if (ep.resid != nullptr && row_ok) {   // one bf16 rounding of acc + bias + R: the residual add of a CLIP layer
+            const uint4* rp = reinterpret_cast<const uint4*>(ep.resid + static_cast<long long>(row) * ep.ldr + col0 + sub * kSubPairs * 2);
+#pragma unroll
+            for (int g = 0; g < kSubPairs / 4; ++g) {
+              const uint4 r4 = rp[g];
+              v[4 * g] = add2(v[4 * g], pk2(bf16_lo(r4.x), bf16_hi(r4.x)));
+              v[4 * g + 1] = add2(v[4 * g + 1], pk2(bf16_lo(r4.y), bf16_hi(r4.y)));
+              v[4 * g + 2] = add2(v[4 * g + 2], pk2(bf16_lo(r4.z), bf16_hi(r4.z)));
+              v[4 * g + 3] = add2(v[4 * g + 3], pk2(bf16_lo(r4.w), bf16_hi(r4.w)));
+            }
+          }
+          if (ep.gelu == 2) {
+#pragma unroll
+            for (int j = 0; j < kSubPairs; ++j) v[j] = quick_gelu_pk(v[j]);
+          }
+        } else if (ep.gelu) {
 #pragma unroll
           for (int j = 0; j < kSubPairs; ++j) v[j] = gelu_erf_pk(v[j]);
         }
@@ -382,12 +413,12 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
         }
       }
     }
-    if (chunk == kChunks - 1 && ep.stats_out != nullptr && row_ok) {
+    if (chunk == kChunks - 1 && !kTower && ep.stats_out != nullptr && row_ok) {
       // statistics are final once the last chunk's values exist; written BEFORE the last slab is handed over so that the store
       // warp's tile-done release (dependent GEMMs of the same launch read them) covers these stores too
       const int slot = (col_tile0 + half * kColsPerWarp) / kColsPerWarp;
       long long srow = row;
-      if (ep.wm_s != 0) srow = window_major_row(row, ep.wm_s);
+      if (!kTower && ep.wm_s != 0) srow = window_major_row(row, ep.wm_s);
       if (slot < ep.stats_out_slots) {
         // (mean, M2) of this 128-column block: mean = shift + s1/n, M2 = s2 - s1^2/n  (deviations from `shift` are O(std): no cancellation)
         constexpr float inv_n = 1.0f / kColsPerWarp;
@@ -556,7 +587,7 @@ struct GemmConfig {
   static_assert(kSmemBytes <= 232448, "shared memory budget of an sm_90 SM (227 KiB)");
 };
 
-template <int kBlockN>
+template <int kBlockN, bool kTower = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
                int a_seg_rows, GemmEpilogue ep) {
@@ -642,8 +673,8 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, half * kN * kBlockK * 2, full_bar, empty_bar, kStages, stage, phase,
                          num_k_blocks);
       const OutStage no_stage{nullptr, nullptr, nullptr, 0u};
-      epilogue_tile<kBlockN>(ep, M, N, acc, scratch, m_blk * kBlockM + epi_row(quarter, lane), n_blk * kBlockN, quarter, half, s_col,
-                             no_stage);
+      epilogue_tile<kBlockN, kTower>(ep, M, N, acc, scratch, m_blk * kBlockM + epi_row(quarter, lane), n_blk * kBlockN, quarter, half, s_col,
+                                     no_stage);
     }
   }
 }
@@ -776,6 +807,7 @@ __device__ __forceinline__ TileRef decode_tile(const GemmGroup& g, int tile) {
   return t;
 }
 
+template <bool kTower = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ PeerStores peers) {
   using Cfg = Gemm2Config;
@@ -839,7 +871,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
     uint32_t phase = 0;
     uint32_t slab_seq = 0;
     float acc[2][kN / 2];
-    if (grp.front.x0 != nullptr) {
+    if (!kTower && grp.front.x0 != nullptr) {
       // point queries: this CTA's share of the (query, 8-channel vector) items, 128 vectors per query
       const FrontWork& fw = grp.front;
       const int g = 24 / fw.s, mq = g * g;
@@ -880,7 +912,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       float* s_col = s_col_base;
       const int row_tile0 = t.m_blk * Cfg::kTileM + static_cast<int>(cta_rank) * kBlockM;
       const int row = row_tile0 + epi_row(quarter, lane);
-      if (pr.kind == 1) {
+      if (!kTower && pr.kind == 1) {
         const AttnParams& at = pr.attn;
         const int head = t.n_blk * 2 + half;                 // column half == head of the tile's pair
         GemmEpilogue vec;                                    // only col_a / col_b are read by the staging helper
@@ -905,17 +937,17 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       }
       stage_col_vectors<kTileN>(pr.ep, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
       const int n_kb = t.kb1 - t.kb0;
-      if (pr.ab_mn_major == 1)
+      if (!kTower && pr.ab_mn_major == 1)
         mma_tile<kN, 1, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
-      else if (pr.ab_mn_major == 2)
+      else if (!kTower && pr.ab_mn_major == 2)
         mma_tile<kN, 0, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
       else
         mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
       const OutStage out{pr.use_tma_store ? s_out + half * Cfg::kOutBufs * kOutSlabBytes : nullptr, slab_full_bar + half * Cfg::kOutBufs,
                          slab_empty_bar + half * Cfg::kOutBufs, slab_seq};
       if (pr.use_tma_store) slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);     // slabs per tile and column half
-      epilogue_tile<kTileN>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, quarter, half, s_col, out,
-                            static_cast<long long>(t.split) * pr.c_split_stride);
+      epilogue_tile<kTileN, kTower>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, quarter, half, s_col, out,
+                                    static_cast<long long>(t.split) * pr.c_split_stride);
     }
   } else {
     setmaxnreg_dec<kAuxRegs>();

@@ -1,0 +1,139 @@
+"""The frozen CLIP-ViT-L/14-336 vision tower on the sm_90a kernels (include/tokenpacker_b200_clip_tower.h).
+
+``CLIPVisionTowerB200(clip_vision_model).hidden_states(crops)`` returns hidden states 12, 16, 22 and 23 of transformers'
+``CLIPVisionModel`` — exactly what ``TokenPackerB200.forward_hidden_states`` takes — without running layer 23 or post_layernorm
+and without keeping the other 21 hidden states alive.  The reference's ``encode_images`` becomes
+
+    proj.forward_hidden_states(tower.hidden_states(crops))          # or forward_hidden_states_packed for the HD 'slice' path
+
+transformers is never imported: any module with CLIPVisionModel's parameter names (with or without the ``vision_model.`` prefix)
+and a ``.config`` carrying its fields is accepted.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import warnings
+
+import torch
+from torch import nn
+
+from . import _lib
+from ._lib import check, lib
+
+_TOKENS = 577
+_IMAGE = 336
+_OUT_LAYERS = (12, 16, 22, 23)
+
+
+def _check_config(cfg):
+    want = {"hidden_size": 1024, "intermediate_size": 4096, "num_attention_heads": 16, "patch_size": 14, "image_size": 336,
+            "hidden_act": "quick_gelu", "num_channels": 3}
+    if cfg is None:
+        raise NotImplementedError("the vision model has no .config: CLIP-ViT-L/14-336 (CLIPVisionConfig) is required")
+    for key, value in want.items():
+        got = getattr(cfg, key, None)
+        if got != value:
+            raise NotImplementedError(f"CLIPVisionTowerB200 runs CLIP-ViT-L/14-336 only: config.{key} = {got!r}, expected {value!r}")
+    layers = getattr(cfg, "num_hidden_layers", 0)
+    if not isinstance(layers, int) or layers < _lib.CLIP_TOWER_LAYERS:
+        raise NotImplementedError(f"config.num_hidden_layers = {layers!r}: hidden_states[23] needs at least 23 layers")
+    eps = getattr(cfg, "layer_norm_eps", None)
+    if not isinstance(eps, float) or abs(eps - 1e-5) > 1e-12:
+        raise NotImplementedError(f"config.layer_norm_eps = {eps!r}, expected 1e-5")
+
+
+class CLIPVisionTowerB200(nn.Module):
+    """Forward-only CLIPVisionModel (openai/clip-vit-large-patch14-336) up to hidden_states[23].
+
+    The wrapped model stays the owner of the parameters (``self.vision_model``).  A derived cache (about 147 MB: per layer the q/k/v
+    concatenation with q scaled by 1/8, and the biases in fp32) is keyed on every parameter's ``(data_ptr, _version, dtype)``
+    and dropped by ``load_state_dict``, ``.to()`` / ``.cuda()`` / ``.half()`` and ``invalidate_packed()``.  fp16 / fp32 towers are cast
+    to bf16 once, with a warning."""
+
+    def __init__(self, vision_model: nn.Module):
+        super().__init__()
+        _check_config(getattr(vision_model, "config", None))
+        named = dict(vision_model.named_parameters())
+        prefix = "vision_model." if "vision_model.embeddings.class_embedding" in named else ""
+        names = [prefix + key for _, key in _lib.CLIP_TOWER_FIELDS]
+        for i in range(_lib.CLIP_TOWER_LAYERS):
+            names += [f"{prefix}encoder.layers.{i}.{key}" for _, key in _lib.CLIP_TOWER_LAYER_FIELDS]
+        missing = [n for n in names if n not in named]
+        if missing:
+            raise NotImplementedError(f"not a CLIPVisionModel: parameters {missing[:3]} are missing")
+        self.vision_model = vision_model
+        self._names = names
+        self._packed = None
+        self._packed_key = None
+        self._weights = None
+        self._warned_dtype = False
+        self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
+
+    def invalidate_packed(self):
+        """Drop the derived weight cache (call it after writing parameters through a ``.data`` alias: such writes change neither
+        ``data_ptr`` nor ``_version``)."""
+        self._packed = None
+        self._packed_key = None
+        self._weights = None
+
+    def _apply(self, fn, *args, **kwargs):
+        self.invalidate_packed()
+        return super()._apply(fn, *args, **kwargs)
+
+    def _params(self):
+        named = dict(self.vision_model.named_parameters())
+        return [named[n] for n in self._names]
+
+    def _packed_weights(self, device):
+        params = self._params()
+        key = (str(device),) + tuple((p.data_ptr(), p._version, p.dtype) for p in params)
+        if self._packed is not None and self._packed_key == key:
+            return self._packed, self._weights
+        if any(p.dtype != torch.bfloat16 for p in params) and not self._warned_dtype:
+            self._warned_dtype = True
+            warnings.warn("CLIPVisionTowerB200 computes with bf16 storage and fp32 accumulation: the tower's fp16 / fp32 parameters are "
+                          "cast to bf16 once into the derived cache", UserWarning, stacklevel=3)
+        # bf16 parameters are read in place; anything else (other dtype, non-contiguous, not 16-byte aligned) through a bf16 copy
+        bf = [p.detach().to(device=device, dtype=torch.bfloat16).contiguous() for p in params]
+        bf = [t if t.data_ptr() % 16 == 0 else t.clone() for t in bf]
+        n_top = len(_lib.CLIP_TOWER_FIELDS)
+        w = _lib.TpClipTowerWeights(*[t.data_ptr() for t in bf[:n_top]])
+        per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
+        for i in range(_lib.CLIP_TOWER_LAYERS):
+            w.layers[i] = _lib.TpClipTowerLayer(*[t.data_ptr() for t in bf[n_top + i * per: n_top + (i + 1) * per]])
+        nbytes = lib.tp_clip_tower_packed_bytes()
+        packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        stream = torch.cuda.current_stream(device).cuda_stream
+        check(lib.tp_clip_tower_pack_weights(C.byref(w), packed.data_ptr(), nbytes, stream), "tp_clip_tower_pack_weights")
+        # bf16 parameters are read in place by every forward; the cast copies of other dtypes are kept alive with the cache
+        self._packed, self._packed_key, self._weights = packed, key, (w, bf)
+        return packed, self._weights
+
+    def hidden_states(self, images: torch.Tensor):
+        """images: [N, 3, 336, 336] CUDA crops (bf16 read in place, any crop stride; other dtypes cast to bf16).  Returns the tuple
+        (hidden_states[12], [16], [22], [23]), each bf16 [N, 577, 1024] with the CLS row."""
+        if not isinstance(images, torch.Tensor) or images.dim() != 4 or tuple(images.shape[1:]) != (3, _IMAGE, _IMAGE):
+            shape = tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__
+            raise ValueError(f"expected crops [N,3,336,336], got {shape}")
+        if torch.is_grad_enabled() and (images.requires_grad or any(p.requires_grad for p in self._params())):
+            raise NotImplementedError("CLIPVisionTowerB200 is forward only (the tower is frozen in every TokenPacker recipe): run it under "
+                                      "torch.no_grad(), or detach the crops and freeze the tower's parameters")
+        if not images.is_cuda:
+            raise RuntimeError("tokenpacker_b200 has no CPU path: crops must be CUDA tensors on an H100")
+        n = images.shape[0]
+        device = images.device
+        outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=torch.bfloat16, device=device) for _ in _OUT_LAYERS)
+        if n == 0:
+            return outs
+        with torch.cuda.device(device):
+            x = images.to(torch.bfloat16)
+            if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
+                x = x.contiguous()
+            packed, (w, _) = self._packed_weights(device)
+            ws_bytes = lib.tp_clip_tower_workspace_bytes(n)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+            ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
+            stream = torch.cuda.current_stream(device).cuda_stream
+            check(lib.tp_clip_tower_forward(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), ptrs, ws.data_ptr(), ws_bytes, stream),
+                  "tp_clip_tower_forward")
+        return outs
