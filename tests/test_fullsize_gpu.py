@@ -166,6 +166,7 @@ def test_packed_rows_pair_kernel_bit_exact(s, hidden, monkeypatch):
 def test_arbitrary_row_offsets_still_supported(monkeypatch):
     """tp_forward's seg_row_offset form (arbitrary destination rows, direct stores) is kept: scatter crops in REVERSE order.
     (That form runs the separate-kernel plan, so the dense reference is taken from the same plan: TP_FUSE_ATTN=0.)"""
+    from tokenpacker_b200._lib import lib
     monkeypatch.setenv("TP_FUSE_ATTN", "0")
     m, _ = _module(512, 4, seed=4)
     x0, xm = _inputs(5, 3)
@@ -173,7 +174,11 @@ def test_arbitrary_row_offsets_still_supported(monkeypatch):
         dense = m((x0, xm))
         seg = torch.tensor([(4 - i) * 40 for i in range(5)], dtype=torch.int64, device="cuda")
         out = torch.zeros(5 * 40, 512, dtype=torch.bfloat16, device="cuda")
-        m._launch(x0, x0.stride(0), xm, xm.stride(0), out, seg)
+        ws_bytes = lib.tp_workspace_bytes(5, 4, 512)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device="cuda")
+        st = lib.tp_forward(m._packed_weights(x0.device).data_ptr(), x0.data_ptr(), xm.data_ptr(), 5, x0.stride(0), xm.stride(0), 4, 512,
+                            out.data_ptr(), seg.data_ptr(), ws.data_ptr(), ws_bytes, torch.cuda.current_stream().cuda_stream)
+        assert st == 0, lib.tp_strerror(st)
     for i in range(5):
         assert torch.equal(out[(4 - i) * 40:(4 - i) * 40 + 36], dense[i])
 

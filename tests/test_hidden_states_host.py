@@ -126,3 +126,25 @@ def test_python_refuses_bad_input_before_device_work():
         m.input_grad = False
         with pytest.raises(RuntimeError, match="no CPU path"):
             m.forward_hidden_states(g)
+
+
+def test_forward_layers_refuses_bad_input_before_device_work():
+    """forward_layers is inference only and checks its layers itself: training mode is refused first, then the layer count and
+    each layer's shape and device, CPU tensors included, with ValueError; it has no input_grad refusal."""
+    from tokenpacker_b200 import TokenPackerB200
+    m = TokenPackerB200(hidden_size=256, scale_factor=2)
+    hs = [torch.zeros(1, 577, 1024) for _ in range(4)]
+    with pytest.raises(NotImplementedError, match="inference path"):
+        m.forward_layers(hs[:3])                                      # trainable parameters under autograd, whatever the layers
+    with torch.no_grad():
+        with pytest.raises(ValueError, match="4 hidden states"):
+            m.forward_layers(hs[:3])
+        for bad in (torch.zeros(1, 575, 1024), torch.zeros(1, 577, 4096), torch.zeros(577, 1024)):
+            with pytest.raises(ValueError, match="CUDA tensor"):
+                m.forward_layers(hs[:3] + [bad])
+        with pytest.raises(ValueError, match="CUDA tensor"):
+            m.forward_layers(hs)                                      # CPU layers: ValueError here, not the RuntimeError of forward()
+    m.requires_grad_(False)
+    g = [t.clone().requires_grad_(True) for t in hs]
+    with pytest.raises(ValueError, match="CUDA tensor"):
+        m.forward_layers(g)                                           # layers that require grad are not refused for input_grad

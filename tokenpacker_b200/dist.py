@@ -117,26 +117,18 @@ class FusedGatherTokenPacker:
     def forward_hd(self, x_local, counts: Sequence[int], h_block, w_block, sep_row, ret_row):
         """HD path across ranks in ONE pass: returns (packed [sum(L_i), H], cu_seqlens) — the packed tensor is a view of a
         symmetric buffer that stays valid until the call after next."""
-        from ._lib import lib, check
-        from .hd import hd_plan_device
+        from .hd import fill_separators, hd_layout
         proj = self.projector
         rank = dist.get_rank(self.group)
         device = x_local[0].device
         m, hidden = proj.num_queries, proj.hidden_size
-        plan, _, sep_rows, ret_rows = hd_plan_device(h_block, w_block, m, device)
         total_crops = int(sum(counts))
-        if plan.n_crops != total_crops:
-            raise ValueError(f"grids describe {plan.n_crops} crops but the ranks hold {total_crops}")
-        total_rows = int(plan.cu_seqlens[-1])
+        plan, _, sep_rows, ret_rows, total_rows = hd_layout(h_block, w_block, m, device, total_crops, "the ranks hold {}")
         assert total_rows == total_crops * (m + 1)
         buf, hdl = self._buffers((total_rows, hidden), device)
         with torch.cuda.device(device):
             # separator rows of MY copy (local stores; peers only ever write crop rows)
-            sep_b = sep_row.to(device=device, dtype=torch.bfloat16).contiguous()
-            ret_b = ret_row.to(device=device, dtype=torch.bfloat16).contiguous()
-            stream = torch.cuda.current_stream(device).cuda_stream
-            check(lib.tp_hd_fill_separators(buf.data_ptr(), hidden, sep_rows.data_ptr(), sep_rows.numel(), sep_b.data_ptr(),
-                                            ret_rows.data_ptr(), ret_rows.numel(), ret_b.data_ptr(), stream), "tp_hd_fill_separators")
+            fill_separators(buf, sep_row, ret_row, sep_rows, ret_rows)
         if counts[rank] > 0:
             proj.forward_into_peers(x_local, list(hdl.buffer_ptrs), int(sum(counts[:rank])), out_crop_rows=m + 1)
         hdl.barrier(channel=0)          # every rank's stores have landed everywhere

@@ -294,6 +294,59 @@ def hd_plan_device(h_block, w_block, tokens_per_crop: int, device):
     return hit
 
 
+def hd_layout(h_block, w_block, tokens_per_crop: int, device, n_crops: int, given: str = "{} were given"):
+    """hd_plan_device checked against the ``n_crops`` crops the caller holds (``given`` words them in the error).  Returns (plan,
+    seg_row_offset, sep_rows, ret_rows, total packed rows), the index tensors on ``device``."""
+    plan, seg, sep_rows, ret_rows = hd_plan_device(h_block, w_block, tokens_per_crop, device)
+    if plan.n_crops != n_crops:
+        raise ValueError(f"grids describe {plan.n_crops} crops but " + given.format(n_crops))
+    return plan, seg, sep_rows, ret_rows, int(plan.cu_seqlens[-1])
+
+
+def fill_separators(out: torch.Tensor, sep_row: torch.Tensor, ret_row: torch.Tensor, sep_rows: torch.Tensor, ret_rows: torch.Tensor):
+    """Write the ',' embedding ``sep_row`` into rows ``sep_rows`` and the '\\n' embedding ``ret_row`` into rows ``ret_rows`` of the
+    packed bf16 [rows, H] ``out`` (tp_hd_fill_separators, on the current stream of out's device)."""
+    device = out.device
+    sep_b = sep_row.to(device=device, dtype=torch.bfloat16).contiguous()
+    ret_b = ret_row.to(device=device, dtype=torch.bfloat16).contiguous()
+    check(lib.tp_hd_fill_separators(out.data_ptr(), out.shape[1], sep_rows.data_ptr(), sep_rows.numel(), sep_b.data_ptr(),
+                                    ret_rows.data_ptr(), ret_rows.numel(), ret_b.data_ptr(), torch.cuda.current_stream(device).cuda_stream),
+          "tp_hd_fill_separators")
+
+
+class _PackedScatterFunction(torch.autograd.Function):
+    """Differentiable slice assembly (llava_arch.py:139-155) for the training path: crop blocks [N,M,H] -> packed rows, with the
+    ',' / '\\n' rows filled in.  Forward = tp_hd_scatter_crops + tp_hd_fill_separators; backward = one row gather
+    (tp_gather_rows with the forward's destination rows as source index) plus the column sums of the separator rows' gradients."""
+
+    @staticmethod
+    def forward(ctx, feats, sep_row, ret_row, seg, sep_rows, ret_rows, total_rows):
+        n, m, h = feats.shape
+        fb = feats.contiguous()
+        out = torch.empty((total_rows, h), dtype=torch.bfloat16, device=feats.device)
+        stream = torch.cuda.current_stream(feats.device).cuda_stream
+        check(lib.tp_hd_scatter_crops(fb.data_ptr(), n, m, h, seg.data_ptr(), out.data_ptr(), stream), "tp_hd_scatter_crops")
+        fill_separators(out, sep_row, ret_row, sep_rows, ret_rows)
+        ctx.shape = (n, m, h)
+        ctx.meta = (sep_row.dtype, ret_row.dtype)
+        ctx.save_for_backward(seg, sep_rows, ret_rows)
+        return out
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        seg, sep_rows, ret_rows = ctx.saved_tensors
+        n, m, h = ctx.shape
+        g = g.to(torch.bfloat16).contiguous()
+        src = (seg.view(n, 1) + torch.arange(m, device=g.device, dtype=torch.int64).view(1, m)).reshape(-1).contiguous()
+        gf = torch.empty((n * m, h), dtype=torch.bfloat16, device=g.device)
+        stream = torch.cuda.current_stream(g.device).cuda_stream
+        check(lib.tp_gather_rows(g.data_ptr(), g.data_ptr(), h, src.data_ptr(), n * m, gf.data_ptr(), stream), "tp_gather_rows")
+        g_sep = g.index_select(0, sep_rows).float().sum(0).to(ctx.meta[0]) if ctx.needs_input_grad[1] else None
+        g_ret = g.index_select(0, ret_rows).float().sum(0).to(ctx.meta[1]) if ctx.needs_input_grad[2] else None
+        return gf.view(n, m, h), g_sep, g_ret, None, None, None, None
+
+
 def hd_assemble(feats: torch.Tensor, h_block, w_block, sep_row: torch.Tensor, ret_row: torch.Tensor):
     """llava_arch.py:139-155 for already-projected crop features [sum(crops), M, H] (bf16, CUDA).
 
@@ -303,21 +356,15 @@ def hd_assemble(feats: torch.Tensor, h_block, w_block, sep_row: torch.Tensor, re
         raise RuntimeError("tokenpacker_b200 has no CPU path: feats must be a CUDA tensor")
     m, hdim = int(feats.shape[1]), int(feats.shape[2])
     device = feats.device
-    plan, seg, sep_rows, ret_rows = hd_plan_device(h_block, w_block, m, device)
-    if plan.n_crops != feats.shape[0]:
-        raise ValueError(f"grids describe {plan.n_crops} crops but {feats.shape[0]} were given")
+    plan, seg, sep_rows, ret_rows, total = hd_layout(h_block, w_block, m, device, feats.shape[0])
     if torch.is_grad_enabled() and (feats.requires_grad or sep_row.requires_grad or ret_row.requires_grad):
-        from .projector import _PackedScatterFunction      # training: differentiable scatter (gradient = one row gather)
-        with torch.cuda.device(device):
-            out = _PackedScatterFunction.apply(feats.to(torch.bfloat16), sep_row, ret_row, seg, sep_rows, ret_rows, int(plan.cu_seqlens[-1]))
+        with torch.cuda.device(device):      # training: differentiable scatter (gradient = one row gather)
+            out = _PackedScatterFunction.apply(feats.to(torch.bfloat16), sep_row, ret_row, seg, sep_rows, ret_rows, total)
         return (out if feats.dtype == torch.bfloat16 else out.to(feats.dtype)), plan.cu_seqlens
     fb = feats.to(torch.bfloat16).contiguous()
     with torch.cuda.device(device):
-        out = torch.empty((int(plan.cu_seqlens[-1]), hdim), dtype=torch.bfloat16, device=device)
+        out = torch.empty((total, hdim), dtype=torch.bfloat16, device=device)
         stream = torch.cuda.current_stream(device).cuda_stream
         check(lib.tp_hd_scatter_crops(fb.data_ptr(), plan.n_crops, m, hdim, seg.data_ptr(), out.data_ptr(), stream), "tp_hd_scatter_crops")
-        sep_b = sep_row.to(device=device, dtype=torch.bfloat16).contiguous()
-        ret_b = ret_row.to(device=device, dtype=torch.bfloat16).contiguous()
-        check(lib.tp_hd_fill_separators(out.data_ptr(), hdim, sep_rows.data_ptr(), sep_rows.numel(), sep_b.data_ptr(),
-                                        ret_rows.data_ptr(), ret_rows.numel(), ret_b.data_ptr(), stream), "tp_hd_fill_separators")
+        fill_separators(out, sep_row, ret_row, sep_rows, ret_rows)
     return (out if feats.dtype == torch.bfloat16 else out.to(feats.dtype)), plan.cu_seqlens

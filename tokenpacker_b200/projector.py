@@ -17,7 +17,7 @@ import torch
 import torch.nn as nn
 from torch.nn.init import trunc_normal_
 
-from . import _lib
+from . import _lib, hd
 from ._lib import lib, check
 
 _CLIP_LAYERS = 4          # builder.py:61,67: the multi-level stack is 4 CLIP layers x 1024 = 4096 (hard-coded upstream)
@@ -56,155 +56,177 @@ def _pack_train(module, params, device):
     return bf, w_struct, packed
 
 
-class _ProjectorFunction(torch.autograd.Function):
-    """autograd bridge: forward = tp_forward_train (keeps intermediates), backward = tp_backward (parameter gradients), or
-    tp_backward_inputs when x0b / xmb need a gradient too (``TokenPackerB200.input_grad``)."""
-
-    @staticmethod
-    def forward(ctx, module, x0b, s0, xmb, sm, *params):
-        device = x0b.device
-        n = x0b.shape[0]
-        bf, w_struct, packed = _pack_train(module, params, device)
-        stream = torch.cuda.current_stream(device).cuda_stream
-        out = torch.empty((n, module.num_queries, module.hidden_size), dtype=torch.bfloat16, device=device)
-        nbytes = lib.tp_train_saved_bytes(n, module.scale_factor, module.hidden_size)
-        saved = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        check(lib.tp_forward_train(C.byref(w_struct), packed.data_ptr(), x0b.data_ptr(), xmb.data_ptr(), n, s0, sm, module.scale_factor,
-                                   module.hidden_size, out.data_ptr(), saved.data_ptr(), nbytes, stream), "tp_forward_train")
-        ctx.module = module
-        ctx.saved = saved
-        ctx.packed = packed if ctx.needs_input_grad[3] else None     # dxm reads [W_k0; W_v0] from it; ~80 MB at hidden 4096, else dropped
-        ctx.xm = xmb if xmb.is_contiguous() else xmb.contiguous()
-        ctx.weights_bf16 = bf                                # the parameters this forward read (bf16; aliases of the live ones when they are bf16)
-        ctx.param_meta = [(p.dtype, p.requires_grad) for p in params]
-        return out
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, grad_out):
-        module = ctx.module
-        device = grad_out.device
-        n = ctx.xm.shape[0]
-        g = grad_out.to(torch.bfloat16).contiguous()
-        grads = [torch.empty_like(w) for w in ctx.weights_bf16]
-        w_struct = _lib.TpWeights(*[t.data_ptr() for t in ctx.weights_bf16])
-        g_struct = _lib.TpWeights(*[t.data_ptr() for t in grads])
-        need_x0, need_xm = ctx.needs_input_grad[1], ctx.needs_input_grad[3]
-        d_x0 = d_xm = None
-        with torch.cuda.device(device):
-            ws_bytes = lib.tp_backward_workspace_bytes(n, module.scale_factor, module.hidden_size)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            stream = torch.cuda.current_stream(device).cuda_stream
-            if need_x0 or need_xm:
-                d_x0 = torch.empty((n, 576, 1024), dtype=torch.bfloat16, device=device) if need_x0 else None     # every element written
-                d_xm = torch.empty((n, 576, 4096), dtype=torch.bfloat16, device=device) if need_xm else None
-                check(lib.tp_backward_inputs(C.byref(w_struct), ctx.packed.data_ptr() if need_xm else None, ctx.xm.data_ptr(),
-                                             ctx.xm.stride(0), n, module.scale_factor, module.hidden_size, g.data_ptr(), ctx.saved.data_ptr(),
-                                             C.byref(g_struct), d_x0.data_ptr() if need_x0 else None,
-                                             d_xm.data_ptr() if need_xm else None, ws.data_ptr(), ws_bytes, stream), "tp_backward_inputs")
-            else:
-                check(lib.tp_backward(C.byref(w_struct), ctx.xm.data_ptr(), ctx.xm.stride(0), n, module.scale_factor, module.hidden_size,
-                                      g.data_ptr(), ctx.saved.data_ptr(), C.byref(g_struct), ws.data_ptr(), ws_bytes, stream), "tp_backward")
-        out = [gr.to(dt) if need else None for gr, (dt, need) in zip(grads, ctx.param_meta)]
-        return (None, d_x0, None, d_xm, None) + tuple(out)
+def _as_crop_strided(t: torch.Tensor, width: int):
+    """Return (tensor, crop_stride) with unit channel stride and dense rows; [:,1:] CLIP views pass through."""
+    if t.stride(2) == 1 and t.stride(1) == width and t.stride(0) >= 576 * width and t.stride(0) % 8 == 0 \
+            and t.data_ptr() % 16 == 0:
+        return t, t.stride(0)
+    t = t.contiguous()
+    return t, t.stride(0)
 
 
 def _token_rows(layers):
-    """ctypes array of the four layers' token row 0 (after the CLS row of a [N,577,1024] layer)."""
-    return (C.c_void_p * 4)(*[t.data_ptr() + (t.shape[1] - 576) * 1024 * t.element_size() for t in layers])
+    """ctypes array of each [N,577,1024] or [N,576,1024] tensor's token row 0 (after the CLS row), NULL for a None entry."""
+    return (C.c_void_p * 4)(*[t.data_ptr() + (t.shape[1] - 576) * 1024 * t.element_size() if t is not None else None for t in layers])
 
 
-class _HiddenStatesFunction(torch.autograd.Function):
-    """autograd bridge of ``TokenPackerB200.forward_hidden_states``: forward = tp_forward_train_layers, backward = tp_backward_layers,
-    both reading the four bf16 hidden states (each [N,577,1024] or each [N,576,1024], one crop stride) in place.  Layer gradients
-    come back in the layers' shape, CLS rows zero, written by the backward's GEMMs straight into their token rows."""
+class _Features:
+    """The CLIP-feature operand of one projector call, the host counterpart of the library's C ``Features``: the (feat, feat_multi)
+    pair (``_PairFeatures``) or the four hidden states (``_LayerFeatures``), as bf16 tensors the kernels read in place.  ``inputs``
+    are the tensors autograd sees, ``dtype`` is the caller's (results are cast back to it).  The subclasses' methods are the only code
+    that knows the form: which entry points run, with which pointers, what the backward keeps and what input gradients it returns."""
+
+    def __init__(self, inputs, dtype):
+        self.inputs = tuple(inputs)
+        self.dtype = dtype
+        self.n = self.inputs[0].shape[0]
+        self.device = self.inputs[0].device
+
+
+class _PairFeatures(_Features):
+    """(feat [N,576,1024], feat_multi [N,576,4096]), each read through its own crop stride."""
+
+    def __init__(self, x0, xm):
+        x0b, self.s0 = _as_crop_strided(x0.to(torch.bfloat16), 1024)
+        xmb, self.sm = _as_crop_strided(xm.to(torch.bfloat16), 4096)
+        super().__init__((x0b, xmb), x0.dtype)
+
+    def launch(self, m, packed, out, out_crop_rows, ws, ws_bytes, stream):
+        x0b, xmb = self.inputs
+        if out_crop_rows:
+            check(lib.tp_forward_packed(packed.data_ptr(), x0b.data_ptr(), xmb.data_ptr(), self.n, self.s0, self.sm, m.scale_factor,
+                                        m.hidden_size, out.data_ptr(), out_crop_rows, ws.data_ptr(), ws_bytes, stream), "tp_forward_packed")
+        else:
+            check(lib.tp_forward(packed.data_ptr(), x0b.data_ptr(), xmb.data_ptr(), self.n, self.s0, self.sm, m.scale_factor,
+                                 m.hidden_size, out.data_ptr(), None, ws.data_ptr(), ws_bytes, stream), "tp_forward")
+
+    def launch_train(self, m, w_struct, packed, out, saved, nbytes, stream):
+        x0b, xmb = self.inputs
+        check(lib.tp_forward_train(C.byref(w_struct), packed.data_ptr(), x0b.data_ptr(), xmb.data_ptr(), self.n, self.s0, self.sm,
+                                   m.scale_factor, m.hidden_size, out.data_ptr(), saved.data_ptr(), nbytes, stream), "tp_forward_train")
+
+    def keep_for_backward(self, ctx, packed, need):
+        xmb = self.inputs[1]
+        ctx.packed = packed if need[1] else None            # dxm reads [W_k0; W_v0] from it; ~80 MB at hidden 4096, else dropped
+        ctx.xm = xmb if xmb.is_contiguous() else xmb.contiguous()
 
     @staticmethod
-    def forward(ctx, module, l0, l1, l2, l3, *params):
-        layers = (l0, l1, l2, l3)
-        device = l0.device
-        n = l0.shape[0]
+    def launch_backward(ctx, n, w_struct, g, g_struct, ws, ws_bytes, stream, need):
+        """tp_backward_inputs for the input gradients ``need`` asks for, tp_backward when it asks for none.  -> (d_x0, d_xm)"""
+        m, xm = ctx.module, ctx.xm
+        need_x0, need_xm = need
+        if not (need_x0 or need_xm):
+            check(lib.tp_backward(C.byref(w_struct), xm.data_ptr(), xm.stride(0), n, m.scale_factor, m.hidden_size, g.data_ptr(),
+                                  ctx.saved.data_ptr(), C.byref(g_struct), ws.data_ptr(), ws_bytes, stream), "tp_backward")
+            return None, None
+        d_x0 = torch.empty((n, 576, 1024), dtype=torch.bfloat16, device=g.device) if need_x0 else None     # every element written
+        d_xm = torch.empty((n, 576, 4096), dtype=torch.bfloat16, device=g.device) if need_xm else None
+        check(lib.tp_backward_inputs(C.byref(w_struct), ctx.packed.data_ptr() if need_xm else None, xm.data_ptr(), xm.stride(0), n,
+                                     m.scale_factor, m.hidden_size, g.data_ptr(), ctx.saved.data_ptr(), C.byref(g_struct),
+                                     d_x0.data_ptr() if need_x0 else None, d_xm.data_ptr() if need_xm else None, ws.data_ptr(),
+                                     ws_bytes, stream), "tp_backward_inputs")
+        return d_x0, d_xm
+
+
+class _LayerFeatures(_Features):
+    """The four CLIP hidden states 12, 16, 22, 23 (each [N,577,1024] with the CLS row, or [N,576,1024]; one crop stride).  When they
+    are bf16 of one shape whose token rows share a TMA-compatible crop stride (the tower's own [N,577,1024] outputs), the layers
+    themselves are read in place and nothing is copied; else contiguous bf16 [N,576,1024] copies are, whose cast / slice backward
+    autograd carries."""
+
+    def __init__(self, layers):
+        bases = layers
+        views = [t[:, 1:] if t.shape[1] == 577 else t for t in layers] \
+            if all(t.dtype == torch.bfloat16 for t in layers) and len({t.shape[1] for t in layers}) == 1 else None
+        if views is None or not self._in_place(views):
+            bases = views = [(t[:, 1:] if t.shape[1] == 577 else t).to(torch.bfloat16).contiguous() for t in layers]
+        super().__init__(bases, layers[3].dtype)
+        self.stride = views[0].stride(0)
+        self.rows = (C.c_void_p * 4)(*[v.data_ptr() for v in views])      # each layer's token row 0
+
+    @staticmethod
+    def _in_place(views):
+        stride = views[0].stride(0)
+        return stride % 8 == 0 and stride >= 576 * 1024 and all(v.stride(2) == 1 and v.stride(1) == 1024 and v.stride(0) == stride
+                                                                and v.data_ptr() % 16 == 0 for v in views)
+
+    def launch(self, m, packed, out, out_crop_rows, ws, ws_bytes, stream):
+        if out_crop_rows:
+            check(lib.tp_forward_layers_packed(packed.data_ptr(), self.rows, self.n, self.stride, m.scale_factor, m.hidden_size,
+                                               out.data_ptr(), out_crop_rows, ws.data_ptr(), ws_bytes, stream), "tp_forward_layers_packed")
+        else:
+            check(lib.tp_forward_layers(packed.data_ptr(), self.rows, self.n, self.stride, m.scale_factor, m.hidden_size,
+                                        out.data_ptr(), None, ws.data_ptr(), ws_bytes, stream), "tp_forward_layers")
+
+    def launch_train(self, m, w_struct, packed, out, saved, nbytes, stream):
+        check(lib.tp_forward_train_layers(C.byref(w_struct), packed.data_ptr(), self.rows, self.n, self.stride,
+                                          m.scale_factor, m.hidden_size, out.data_ptr(), saved.data_ptr(), nbytes, stream),
+              "tp_forward_train_layers")
+
+    def keep_for_backward(self, ctx, packed, need):
+        ctx.packed = packed if any(need) else None          # the layer gradients read [W_k0; W_v0] from it
+        ctx.save_for_backward(*self.inputs)                  # read again by the backward: an in-place edit before it raises
+
+    @staticmethod
+    def launch_backward(ctx, n, w_struct, g, g_struct, ws, ws_bytes, stream, need):
+        """tp_backward_layers.  -> the wanted layer gradients in the layers' shape, CLS rows zero, written by the backward's GEMMs
+        straight into their token rows."""
+        m, layers = ctx.module, ctx.saved_tensors
+        rows = layers[0].shape[1]
+        d = [None] * 4
+        for i in range(4):
+            if need[i]:
+                d[i] = torch.empty((n, rows, 1024), dtype=torch.bfloat16, device=g.device)     # token rows: every element written
+                if rows == 577:
+                    d[i][:, 0].zero_()
+        check(lib.tp_backward_layers(C.byref(w_struct), ctx.packed.data_ptr() if ctx.packed is not None else None, _token_rows(layers),
+                                     layers[0].stride(0), n, m.scale_factor, m.hidden_size, g.data_ptr(), ctx.saved.data_ptr(),
+                                     C.byref(g_struct), _token_rows(d) if any(need) else None, rows * 1024, ws.data_ptr(), ws_bytes,
+                                     stream), "tp_backward_layers")
+        return d
+
+
+class _TrainFunction(torch.autograd.Function):
+    """autograd bridge of the training forward: forward = the feature operand's training entry point (tp_forward_train or
+    tp_forward_train_layers, keeping intermediates), backward = its backward entry point (parameter gradients, plus the gradients of
+    the inputs that need one when ``TokenPackerB200.input_grad`` is set).  Arguments: module, features, *features.inputs, *params."""
+
+    @staticmethod
+    def forward(ctx, module, features, *tensors):
+        params = tensors[len(features.inputs):]
+        device, n = features.device, features.n
         bf, w_struct, packed = _pack_train(module, params, device)
         stream = torch.cuda.current_stream(device).cuda_stream
         out = torch.empty((n, module.num_queries, module.hidden_size), dtype=torch.bfloat16, device=device)
         nbytes = lib.tp_train_saved_bytes(n, module.scale_factor, module.hidden_size)
         saved = torch.empty(nbytes, dtype=torch.uint8, device=device)
-        check(lib.tp_forward_train_layers(C.byref(w_struct), packed.data_ptr(), _token_rows(layers), n, l0.stride(0), module.scale_factor,
-                                          module.hidden_size, out.data_ptr(), saved.data_ptr(), nbytes, stream), "tp_forward_train_layers")
+        features.launch_train(module, w_struct, packed, out, saved, nbytes, stream)
         ctx.module = module
+        ctx.n = n
+        ctx.backward_form = type(features)                   # not the operand itself: the backward keeps only what keep_for_backward keeps
         ctx.saved = saved
-        ctx.packed = packed if any(ctx.needs_input_grad[1:5]) else None   # the layer gradients read [W_k0; W_v0] from it
-        ctx.weights_bf16 = bf
+        ctx.weights_bf16 = bf                                # the parameters this forward read (bf16; aliases of the live ones when they are bf16)
         ctx.param_meta = [(p.dtype, p.requires_grad) for p in params]
-        ctx.save_for_backward(*layers)                       # read again by the backward: an in-place edit before it raises
+        features.keep_for_backward(ctx, packed, ctx.needs_input_grad[2:2 + len(features.inputs)])
         return out
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
         module = ctx.module
-        layers = ctx.saved_tensors
         device = grad_out.device
-        n, rows = layers[0].shape[0], layers[0].shape[1]
         g = grad_out.to(torch.bfloat16).contiguous()
         grads = [torch.empty_like(w) for w in ctx.weights_bf16]
         w_struct = _lib.TpWeights(*[t.data_ptr() for t in ctx.weights_bf16])
         g_struct = _lib.TpWeights(*[t.data_ptr() for t in grads])
-        need = ctx.needs_input_grad[1:5]
-        d = [None] * 4
         with torch.cuda.device(device):
-            d_ptrs = None
-            if any(need):
-                for i in range(4):
-                    if need[i]:
-                        d[i] = torch.empty((n, rows, 1024), dtype=torch.bfloat16, device=device)     # token rows: every element written
-                        if rows == 577:
-                            d[i][:, 0].zero_()
-                d_ptrs = (C.c_void_p * 4)(*[t.data_ptr() + (rows - 576) * 2048 if t is not None else None for t in d])
-            ws_bytes = lib.tp_backward_workspace_bytes(n, module.scale_factor, module.hidden_size)
+            ws_bytes = lib.tp_backward_workspace_bytes(ctx.n, module.scale_factor, module.hidden_size)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
             stream = torch.cuda.current_stream(device).cuda_stream
-            check(lib.tp_backward_layers(C.byref(w_struct), ctx.packed.data_ptr() if ctx.packed is not None else None, _token_rows(layers),
-                                         layers[0].stride(0), n, module.scale_factor, module.hidden_size, g.data_ptr(), ctx.saved.data_ptr(),
-                                         C.byref(g_struct), d_ptrs, rows * 1024, ws.data_ptr(), ws_bytes, stream), "tp_backward_layers")
-        out = [gr.to(dt) if need_p else None for gr, (dt, need_p) in zip(grads, ctx.param_meta)]
-        return (None, *d) + tuple(out)
-
-
-class _PackedScatterFunction(torch.autograd.Function):
-    """Differentiable slice assembly (llava_arch.py:139-155) for the training path: crop blocks [N,M,H] -> packed rows, with the
-    ',' / '\\n' rows filled in.  Forward = tp_hd_scatter_crops + tp_hd_fill_separators; backward = one row gather
-    (tp_gather_rows with the forward's destination rows as source index) plus the column sums of the separator rows' gradients."""
-
-    @staticmethod
-    def forward(ctx, feats, sep_row, ret_row, seg, sep_rows, ret_rows, total_rows):
-        n, m, h = feats.shape
-        fb = feats.contiguous()
-        out = torch.empty((total_rows, h), dtype=torch.bfloat16, device=feats.device)
-        sep_b = sep_row.detach().to(device=feats.device, dtype=torch.bfloat16).contiguous()
-        ret_b = ret_row.detach().to(device=feats.device, dtype=torch.bfloat16).contiguous()
-        stream = torch.cuda.current_stream(feats.device).cuda_stream
-        check(lib.tp_hd_scatter_crops(fb.data_ptr(), n, m, h, seg.data_ptr(), out.data_ptr(), stream), "tp_hd_scatter_crops")
-        check(lib.tp_hd_fill_separators(out.data_ptr(), h, sep_rows.data_ptr(), sep_rows.numel(), sep_b.data_ptr(),
-                                        ret_rows.data_ptr(), ret_rows.numel(), ret_b.data_ptr(), stream), "tp_hd_fill_separators")
-        ctx.shape = (n, m, h)
-        ctx.meta = (sep_row.dtype, ret_row.dtype)
-        ctx.save_for_backward(seg, sep_rows, ret_rows)
-        return out
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, g):
-        seg, sep_rows, ret_rows = ctx.saved_tensors
-        n, m, h = ctx.shape
-        g = g.to(torch.bfloat16).contiguous()
-        src = (seg.view(n, 1) + torch.arange(m, device=g.device, dtype=torch.int64).view(1, m)).reshape(-1).contiguous()
-        gf = torch.empty((n * m, h), dtype=torch.bfloat16, device=g.device)
-        stream = torch.cuda.current_stream(g.device).cuda_stream
-        check(lib.tp_gather_rows(g.data_ptr(), g.data_ptr(), h, src.data_ptr(), n * m, gf.data_ptr(), stream), "tp_gather_rows")
-        g_sep = g.index_select(0, sep_rows).float().sum(0).to(ctx.meta[0]) if ctx.needs_input_grad[1] else None
-        g_ret = g.index_select(0, ret_rows).float().sum(0).to(ctx.meta[1]) if ctx.needs_input_grad[2] else None
-        return gf.view(n, m, h), g_sep, g_ret, None, None, None, None
+            d = ctx.backward_form.launch_backward(ctx, ctx.n, w_struct, g, g_struct, ws, ws_bytes, stream,
+                                                  ctx.needs_input_grad[2:-len(grads)])
+        out = [gr.to(dt) if need else None for gr, (dt, need) in zip(grads, ctx.param_meta)]
+        return (None, None, *d) + tuple(out)
 
 
 class TokenPackerB200(nn.Module):
@@ -302,22 +324,13 @@ class TokenPackerB200(nn.Module):
         stream = torch.cuda.current_stream(device).cuda_stream
         check(lib.tp_pack_weights(C.byref(w), self.hidden_size, packed.data_ptr(), nbytes, stream), "tp_pack_weights")
         self._keepalive = bf     # sources must outlive the asynchronous packing kernels
-        # a pack made for a training forward is never reused (see _ProjectorFunction.forward): the next call repacks
+        # a pack made for a training forward is never reused (see _TrainFunction.forward): the next call repacks
         self._packed, self._packed_key = packed, (None if fresh else key)
         return packed
 
     # ------------------------------------------------------------------------------------------------------------
     # forward
     # ------------------------------------------------------------------------------------------------------------
-    @staticmethod
-    def _as_crop_strided(t: torch.Tensor, width: int):
-        """Return (tensor, crop_stride) with unit channel stride and dense rows; [:,1:] CLIP views pass through."""
-        if t.stride(2) == 1 and t.stride(1) == width and t.stride(0) >= 576 * width and t.stride(0) % 8 == 0 \
-                and t.data_ptr() % 16 == 0:
-            return t, t.stride(0)
-        t = t.contiguous()
-        return t, t.stride(0)
-
     def _check_inputs(self, x, attn_mask, differentiable: bool = True):
         if attn_mask is not None:
             raise NotImplementedError("attn_mask must be None (the reference's sole caller passes none, llava_arch.py:97)")
@@ -340,43 +353,57 @@ class TokenPackerB200(nn.Module):
                                       "produce them, or detach the features or run under torch.no_grad()")
         return x0, xm
 
-    def _inputs_need_grad(self, x0, xm) -> bool:
-        return self.input_grad and torch.is_grad_enabled() and (x0.requires_grad or xm.requires_grad)
+    def _trains(self, features) -> bool:
+        """Whether the call needs the training path: gradients for a parameter, or (with ``input_grad``) for a feature input."""
+        return torch.is_grad_enabled() and (any(p.requires_grad for p in self._raw_params()) or
+                                            (self.input_grad and any(t.requires_grad for t in features.inputs)))
 
-    def forward(self, x, attn_mask=None):
-        x0, xm = self._check_inputs(x, attn_mask)
-        out_dtype = x0.dtype
-        n = x0.shape[0]
-        device = x0.device
-        if n == 0:
-            return x0.new_empty((0, self.num_queries, self.hidden_size))
-        with torch.cuda.device(device):
-            x0b, s0 = self._as_crop_strided(x0.to(torch.bfloat16), 1024)
-            xmb, sm = self._as_crop_strided(xm.to(torch.bfloat16), 4096)
-            if (torch.is_grad_enabled() and any(p.requires_grad for p in self._raw_params())) or self._inputs_need_grad(x0, xm):
-                # training: same output, intermediates kept, gradients for every parameter (tp_forward_train / tp_backward) and, with
-                # input_grad, for the features that require one (tp_backward_inputs)
-                out = _ProjectorFunction.apply(self, x0b, s0, xmb, sm, *self._raw_params())
-            else:
-                out = torch.empty((n, self.num_queries, self.hidden_size), dtype=torch.bfloat16, device=device)
-                self._launch(x0b, s0, xmb, sm, out, None)
-        return out if out_dtype == torch.bfloat16 else out.to(out_dtype)
-
-    def _launch(self, x0b, s0, xmb, sm, out, seg_row_offset, out_crop_rows: int = 0):
-        device = x0b.device
-        n = x0b.shape[0]
+    def _launch_resources(self, device, n: int):
+        """(packed weights, workspace, its size in bytes, stream) of an inference launch over n crops."""
         packed = self._packed_weights(device)
         ws_bytes = lib.tp_workspace_bytes(n, self.scale_factor, self.hidden_size)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-        stream = torch.cuda.current_stream(device).cuda_stream
-        if out_crop_rows:
-            check(lib.tp_forward_packed(packed.data_ptr(), x0b.data_ptr(), xmb.data_ptr(), n, s0, sm, self.scale_factor,
-                                        self.hidden_size, out.data_ptr(), int(out_crop_rows), ws.data_ptr(), ws_bytes, stream),
-                  "tp_forward_packed")
-            return
-        seg_ptr = seg_row_offset.data_ptr() if seg_row_offset is not None else None
-        check(lib.tp_forward(packed.data_ptr(), x0b.data_ptr(), xmb.data_ptr(), n, s0, sm, self.scale_factor,
-                             self.hidden_size, out.data_ptr(), seg_ptr, ws.data_ptr(), ws_bytes, stream), "tp_forward")
+        return packed, ws, ws_bytes, torch.cuda.current_stream(device).cuda_stream
+
+    def _launch(self, features, out, out_crop_rows: int = 0):
+        """One inference launch: dense [N, M, hidden] into ``out``, or with ``out_crop_rows`` the packed HD rows (crop i from row
+        i * out_crop_rows)."""
+        packed, ws, ws_bytes, stream = self._launch_resources(features.device, features.n)
+        features.launch(self, packed, out, int(out_crop_rows), ws, ws_bytes, stream)
+
+    def _dense(self, features, train: bool):
+        """[N, M, hidden] in the caller's dtype: through _TrainFunction when ``train``, else one inference launch."""
+        if features.n == 0:
+            return torch.empty((0, self.num_queries, self.hidden_size), dtype=features.dtype, device=features.device)
+        if train:
+            # same output, intermediates kept, gradients for every parameter and, with input_grad, for the inputs that require one
+            out = _TrainFunction.apply(self, features, *features.inputs, *self._raw_params())
+        else:
+            out = torch.empty((features.n, self.num_queries, self.hidden_size), dtype=torch.bfloat16, device=features.device)
+            self._launch(features, out)
+        return out if features.dtype == torch.bfloat16 else out.to(features.dtype)
+
+    def _packed_hd(self, features, h_block, w_block, sep_row, ret_row):
+        """Projector + HD slice assembly (llava_arch.py:139-155) for ``forward_packed`` and ``forward_hidden_states_packed``."""
+        plan, seg, sep_rows, ret_rows, total = hd.hd_layout(h_block, w_block, self.num_queries, features.device, features.n)
+        crop_rows = self.num_queries + 1
+        assert total == plan.n_crops * crop_rows      # one separator row per crop: the uniform stride the kernel relies on
+        train = self._trains(features)
+        if train or (torch.is_grad_enabled() and (sep_row.requires_grad or ret_row.requires_grad)):
+            # the dense result as forward() / forward_hidden_states() return it, then the differentiable scatter
+            feats = self._dense(features, train).to(torch.bfloat16)
+            out = hd._PackedScatterFunction.apply(feats, sep_row, ret_row, seg, sep_rows, ret_rows, total)
+        else:
+            out = torch.empty((total, self.hidden_size), dtype=torch.bfloat16, device=features.device)
+            self._launch(features, out, crop_rows)
+            hd.fill_separators(out, sep_row, ret_row, sep_rows, ret_rows)
+        return (out if features.dtype == torch.bfloat16 else out.to(features.dtype)), plan.cu_seqlens
+
+    def forward(self, x, attn_mask=None):
+        x0, xm = self._check_inputs(x, attn_mask)
+        with torch.cuda.device(x0.device):
+            features = _PairFeatures(x0, xm)
+            return self._dense(features, self._trains(features))
 
     def forward_layers(self, layers):
         """Forward from the four CLIP hidden states (layers 12, 16, 22, 23; each [N,577,1024] with the CLS token, or [N,576,1024])
@@ -385,30 +412,13 @@ class TokenPackerB200(nn.Module):
         self._require_inference("forward_layers")
         if len(layers) != 4:
             raise ValueError("expected the 4 hidden states (12, 16, 22, 23)")
-        views = []
         for t in layers:
-            if t.dim() != 3 or t.shape[2] != 1024 or t.shape[1] not in (576, 577) or not t.is_cuda:
-                raise ValueError("each layer must be a CUDA tensor [N,577,1024] or [N,576,1024]")
-            t = t.to(torch.bfloat16)
-            views.append(t[:, 1:] if t.shape[1] == 577 else t)
-        n = views[0].shape[0]
-        stride = views[0].stride(0)
-        for i, v in enumerate(views):
-            if v.shape[0] != n or v.stride(2) != 1 or v.stride(1) != 1024 or v.stride(0) != stride or v.data_ptr() % 16 != 0:
-                views[i] = None
-        if any(v is None for v in views) or stride % 8 != 0:
-            views = [(t[:, 1:] if t.shape[1] == 577 else t).to(torch.bfloat16).contiguous() for t in layers]
-            stride = views[0].stride(0)
-        device = views[0].device
-        with torch.no_grad(), torch.cuda.device(device):
-            packed = self._packed_weights(device)
-            out = torch.empty((n, self.num_queries, self.hidden_size), dtype=torch.bfloat16, device=device)
-            ws_bytes = lib.tp_workspace_bytes(n, self.scale_factor, self.hidden_size)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            arr = (C.c_void_p * 4)(*[v.data_ptr() for v in views])
-            stream = torch.cuda.current_stream(device).cuda_stream
-            check(lib.tp_forward_layers(packed.data_ptr(), arr, n, stride, self.scale_factor, self.hidden_size, out.data_ptr(), None,
-                                        ws.data_ptr(), ws_bytes, stream), "tp_forward_layers")
+            if t.dim() != 3 or t.shape[2] != 1024 or t.shape[1] not in (576, 577) or not t.is_cuda or t.shape[0] != layers[0].shape[0]:
+                raise ValueError("each layer must be a CUDA tensor [N,577,1024] or [N,576,1024], with the same N")
+        with torch.no_grad(), torch.cuda.device(layers[0].device):
+            features = _LayerFeatures(layers)
+            out = torch.empty((features.n, self.num_queries, self.hidden_size), dtype=torch.bfloat16, device=features.device)
+            self._launch(features, out)
         return out
 
     def _check_layers(self, layers):
@@ -426,24 +436,6 @@ class TokenPackerB200(nn.Module):
             raise RuntimeError("tokenpacker_b200 has no CPU path: inputs must be CUDA tensors on an H100")
         return list(layers)
 
-    @staticmethod
-    def _hidden_state_operands(layers):
-        """(bases, token views, crop stride): when the four layers are bf16 of one shape whose token rows share a TMA-compatible crop
-        stride (the tower's own [N,577,1024] outputs), bases are the layers themselves and nothing is copied; else bases = views =
-        contiguous bf16 [N,576,1024] copies, whose cast / slice backward autograd carries."""
-        if all(t.dtype == torch.bfloat16 for t in layers) and len({t.shape[1] for t in layers}) == 1:
-            views = [t[:, 1:] if t.shape[1] == 577 else t for t in layers]
-            stride = views[0].stride(0)
-            if stride % 8 == 0 and stride >= 576 * 1024 and all(v.stride(2) == 1 and v.stride(1) == 1024 and v.stride(0) == stride
-                                                                and v.data_ptr() % 16 == 0 for v in views):
-                return list(layers), views, stride
-        views = [(t[:, 1:] if t.shape[1] == 577 else t).to(torch.bfloat16).contiguous() for t in layers]
-        return views, views, views[0].stride(0)
-
-    def _hidden_states_train(self, layers) -> bool:
-        return torch.is_grad_enabled() and (any(p.requires_grad for p in self._raw_params()) or
-                                            (self.input_grad and any(t.requires_grad for t in layers)))
-
     def forward_hidden_states(self, layers):
         """Forward from the four CLIP hidden states (layers 12, 16, 22, 23: ``hidden_states[l]`` of the tower, each [N,577,1024] with
         the CLS row or [N,576,1024]) -> [N, M, hidden]: ``feature_select`` + ``torch.cat`` (clip_encoder.py:28-44) + ``forward``
@@ -451,55 +443,18 @@ class TokenPackerB200(nn.Module):
         copied feat_multi is ever made) and, with ``input_grad``, give each layer its gradient (layer 23's is the sum of its feat and
         feat_multi paths), in the layer's shape and dtype with zero CLS rows.  Without gradients this is ``forward_layers``."""
         layers = self._check_layers(layers)
-        out_dtype = layers[3].dtype
-        if layers[0].shape[0] == 0:
-            return layers[3].new_empty((0, self.num_queries, self.hidden_size))
-        if not self._hidden_states_train(layers):
-            out = self.forward_layers(layers)
-        else:
-            with torch.cuda.device(layers[0].device):
-                bases, _, _ = self._hidden_state_operands(layers)
-                out = _HiddenStatesFunction.apply(self, *bases, *self._raw_params())
-        return out if out_dtype == torch.bfloat16 else out.to(out_dtype)
+        with torch.cuda.device(layers[0].device):
+            features = _LayerFeatures(layers)
+            return self._dense(features, self._trains(features))
 
     def forward_hidden_states_packed(self, layers, h_block, w_block, sep_row, ret_row):
         """``forward_packed`` from the four CLIP hidden states (as in ``forward_hidden_states``): projector + HD slice assembly
         (llava_arch.py:139-155).  Inference: the last GEMM's TMA stores write the packed rows directly (tp_forward_layers_packed) and a
         tiny kernel fills the separator rows.  Under autograd: ``forward_hidden_states`` plus the differentiable scatter.  Returns
         (packed [sum(L_i), hidden], cu_seqlens int64 [B+1] on the host)."""
-        from .hd import hd_plan_device
         layers = self._check_layers(layers)
-        device = layers[0].device
-        n = layers[0].shape[0]
-        plan, seg, sep_rows, ret_rows = hd_plan_device(h_block, w_block, self.num_queries, device)
-        if plan.n_crops != n:
-            raise ValueError(f"grids describe {plan.n_crops} crops but {n} were given")
-        total = int(plan.cu_seqlens[-1])
-        crop_rows = self.num_queries + 1
-        assert total == plan.n_crops * crop_rows      # one separator row per crop: the uniform stride the kernel relies on
-        training = self._hidden_states_train(layers) or (torch.is_grad_enabled() and (sep_row.requires_grad or ret_row.requires_grad))
-        with torch.cuda.device(device):
-            if training:
-                feats = self.forward_hidden_states(layers).to(torch.bfloat16)
-                out = _PackedScatterFunction.apply(feats, sep_row, ret_row, seg, sep_rows, ret_rows, total)
-            else:
-                with torch.no_grad():
-                    _, views, stride = self._hidden_state_operands(layers)
-                    packed = self._packed_weights(device)
-                    out = torch.empty((total, self.hidden_size), dtype=torch.bfloat16, device=device)
-                    ws_bytes = lib.tp_workspace_bytes(n, self.scale_factor, self.hidden_size)
-                    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-                    stream = torch.cuda.current_stream(device).cuda_stream
-                    arr = (C.c_void_p * 4)(*[v.data_ptr() for v in views])
-                    check(lib.tp_forward_layers_packed(packed.data_ptr(), arr, n, stride, self.scale_factor, self.hidden_size,
-                                                       out.data_ptr(), crop_rows, ws.data_ptr(), ws_bytes, stream), "tp_forward_layers_packed")
-                    sep_b = sep_row.to(device=device, dtype=torch.bfloat16).contiguous()
-                    ret_b = ret_row.to(device=device, dtype=torch.bfloat16).contiguous()
-                    check(lib.tp_hd_fill_separators(out.data_ptr(), self.hidden_size, sep_rows.data_ptr(), sep_rows.numel(),
-                                                    sep_b.data_ptr(), ret_rows.data_ptr(), ret_rows.numel(), ret_b.data_ptr(), stream),
-                          "tp_hd_fill_separators")
-        out_dtype = layers[3].dtype
-        return (out if out_dtype == torch.bfloat16 else out.to(out_dtype)), plan.cu_seqlens
+        with torch.cuda.device(layers[0].device):
+            return self._packed_hd(_LayerFeatures(layers), h_block, w_block, sep_row, ret_row)
 
     def _require_inference(self, what: str):
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
@@ -514,17 +469,12 @@ class TokenPackerB200(nn.Module):
         barrier must follow.  Inference only."""
         self._require_inference("forward_into_peers")
         x0, xm = self._check_inputs(x, None, differentiable=False)
-        device = x0.device
-        with torch.cuda.device(device):
-            x0b, s0 = self._as_crop_strided(x0.to(torch.bfloat16), 1024)
-            xmb, sm = self._as_crop_strided(xm.to(torch.bfloat16), 4096)
-            n = x0b.shape[0]
-            packed = self._packed_weights(device)
-            ws_bytes = lib.tp_workspace_bytes(n, self.scale_factor, self.hidden_size)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            stream = torch.cuda.current_stream(device).cuda_stream
+        with torch.cuda.device(x0.device):
+            f = _PairFeatures(x0, xm)
+            (x0b, xmb), n = f.inputs, f.n
+            packed, ws, ws_bytes, stream = self._launch_resources(f.device, n)
             arr = (C.c_void_p * len(peer_ptrs))(*[int(p) for p in peer_ptrs])
-            check(lib.tp_forward_allgather(packed.data_ptr(), x0b.data_ptr(), xmb.data_ptr(), n, s0, sm, self.scale_factor,
+            check(lib.tp_forward_allgather(packed.data_ptr(), x0b.data_ptr(), xmb.data_ptr(), n, f.s0, f.sm, self.scale_factor,
                                            self.hidden_size, arr, len(peer_ptrs), int(crop_offset), int(out_crop_rows), ws.data_ptr(),
                                            ws_bytes, stream),
                   "tp_forward_allgather")
@@ -546,14 +496,11 @@ class TokenPackerB200(nn.Module):
         if out is None:
             out = torch.empty((n, self.num_queries, self.hidden_size), dtype=torch.bfloat16).pin_memory()
         with torch.cuda.device(device):
-            packed = self._packed_weights(device)
             chunk = max(1, min(int(chunk_crops), n))
+            packed, ws, ws_bytes, stream = self._launch_resources(device, chunk)
             d_x0 = torch.empty((n, 576, 1024), dtype=torch.bfloat16, device=device)
             d_xm = torch.empty((n, 576, 4096), dtype=torch.bfloat16, device=device)
             d_out = torch.empty((n, self.num_queries, self.hidden_size), dtype=torch.bfloat16, device=device)
-            ws_bytes = lib.tp_workspace_bytes(chunk, self.scale_factor, self.hidden_size)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            stream = torch.cuda.current_stream(device).cuda_stream
             check(lib.tp_forward_host(packed.data_ptr(), x0.data_ptr(), xm.data_ptr(), n, self.scale_factor, self.hidden_size,
                                       out.data_ptr(), d_x0.data_ptr(), d_xm.data_ptr(), d_out.data_ptr(), ws.data_ptr(), ws_bytes,
                                       chunk, stream), "tp_forward_host")
@@ -568,33 +515,9 @@ class TokenPackerB200(nn.Module):
         there directly (tp_forward_packed); the separator rows are filled by a tiny kernel.  Under autograd (training,
         pretrain_hd.sh / finetune_hd.sh use mode='slice') the same result comes from the differentiable forward plus a
         differentiable scatter.  Returns (packed [sum(L_i), hidden], cu_seqlens int64 [B+1] on the host)."""
-        from .hd import hd_plan_device
         x0, xm = self._check_inputs(x, None)
-        device = x0.device
-        plan, seg, sep_rows, ret_rows = hd_plan_device(h_block, w_block, self.num_queries, device)
-        if plan.n_crops != x0.shape[0]:
-            raise ValueError(f"grids describe {plan.n_crops} crops but {x0.shape[0]} were given")
-        total = int(plan.cu_seqlens[-1])
-        crop_rows = self.num_queries + 1
-        assert total == plan.n_crops * crop_rows      # one separator row per crop: the uniform stride the kernel relies on
-        training = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters()) or sep_row.requires_grad
-                                                or ret_row.requires_grad or self._inputs_need_grad(x0, xm))
-        with torch.cuda.device(device):
-            if training:
-                feats = self.forward((x0, xm)).to(torch.bfloat16)
-                out = _PackedScatterFunction.apply(feats, sep_row, ret_row, seg, sep_rows, ret_rows, total)
-            else:
-                x0b, s0 = self._as_crop_strided(x0.to(torch.bfloat16), 1024)
-                xmb, sm = self._as_crop_strided(xm.to(torch.bfloat16), 4096)
-                out = torch.empty((total, self.hidden_size), dtype=torch.bfloat16, device=device)
-                self._launch(x0b, s0, xmb, sm, out, None, out_crop_rows=crop_rows)
-                sep_b = sep_row.to(device=device, dtype=torch.bfloat16).contiguous()
-                ret_b = ret_row.to(device=device, dtype=torch.bfloat16).contiguous()
-                stream = torch.cuda.current_stream(device).cuda_stream
-                check(lib.tp_hd_fill_separators(out.data_ptr(), self.hidden_size, sep_rows.data_ptr(), sep_rows.numel(),
-                                                sep_b.data_ptr(), ret_rows.data_ptr(), ret_rows.numel(), ret_b.data_ptr(), stream),
-                      "tp_hd_fill_separators")
-        return (out if x0.dtype == torch.bfloat16 else out.to(x0.dtype)), plan.cu_seqlens
+        with torch.cuda.device(x0.device):
+            return self._packed_hd(_PairFeatures(x0, xm), h_block, w_block, sep_row, ret_row)
 
     def extra_repr(self):
         return f"scale_factor={self.scale_factor}, num_queries={self.num_queries}, hidden_size={self.hidden_size}, backend=sm_90a"
