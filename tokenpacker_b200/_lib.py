@@ -2,7 +2,8 @@
 
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
 Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
-include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h and include/tokenpacker_b200_clip_tower.h one to one.
+include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h, include/tokenpacker_b200_clip_tower.h and
+include/tokenpacker_b200_clip_tower_f16.h one to one.
 """
 from __future__ import annotations
 
@@ -180,6 +181,15 @@ CLIP_TOWER_SIGNATURES = {
                                         C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
+# the same for include/tokenpacker_b200_clip_tower_f16.h (the tower in fp16, as the evaluation and serving scripts run it)
+TP_CLIP_CROPS_BF16 = 1
+TP_CLIP_CROPS_F16 = 2
+CLIP_TOWER_F16_SIGNATURES = {
+    "tp_clip_tower_pack_weights_f16": (C.c_int, [C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "tp_clip_tower_forward_f16": (C.c_int, [C.c_void_p, C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_int, C.c_int64, C.c_int64,
+                                            C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_void_p]),
+}
+
 
 def _load():
     if not os.path.exists(LIB_PATH):
@@ -188,7 +198,7 @@ def _load():
             "(or `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
-                                      **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES}.items():
+                                      **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

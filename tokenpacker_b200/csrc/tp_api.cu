@@ -13,6 +13,7 @@
 
 #include "../../include/tokenpacker_b200.h"
 #include "../../include/tokenpacker_b200_clip_tower.h"
+#include "../../include/tokenpacker_b200_clip_tower_f16.h"
 #include "../../include/tokenpacker_b200_clip_u8.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"
@@ -210,7 +211,7 @@ struct GemmItem {
 };
 constexpr int kDepFront = -2;      // GemmItem::dep: the A operand is the point-query output of the launch's front work
 
-bool tower_epilogue(const GemmEpilogue& ep);
+int gemm_variant(const GemmEpilogue& ep);
 
 int check_item(const GemmItem& it) {
   if (it.kind == 1) return (it.M > 0 && it.M % 16 == 0 && it.attn.qp != nullptr && it.attn.ctx != nullptr) ? TP_OK : TP_ERR_INVALID_ARGUMENT;
@@ -221,9 +222,9 @@ int check_item(const GemmItem& it) {
   if (it.ep.stats_out != nullptr && (it.N % 256 != 0 || it.ep.stats_out_slots != it.N / 128)) return TP_ERR_INVALID_ARGUMENT;
   if (it.ep.col_a != nullptr && (it.ep.stats_in == nullptr || it.ep.stats_in_slots <= 0)) return TP_ERR_INVALID_ARGUMENT;
   if ((it.b_parts != 1 || it.b_seg_rows != 0) && it.tn != 1) return TP_ERR_INVALID_ARGUMENT;
-  // the tower's epilogue instantiations (tower_epilogue) have no erf GELU, LayerNorm fold, row statistics, dual, window-major or fp32
+  // the tower's epilogue instantiations (gemm_variant 1 and 2) have no erf GELU, LayerNorm fold, row statistics, dual, window-major or fp32
   // output, no KV-attention tiles and no TN / NN operand forms; R is read 16 bytes at a time
-  if (tower_epilogue(it.ep) && (it.ep.gelu == 1 || it.ep.col_a != nullptr || it.ep.stats_out != nullptr || it.ep.dual || it.ep.wm_s != 0 ||
+  if (gemm_variant(it.ep) != 0 && (it.ep.gelu == 1 || it.ep.col_a != nullptr || it.ep.stats_out != nullptr || it.ep.dual || it.ep.wm_s != 0 ||
                                 it.k_splits != 1 || it.kind != 0 || it.tn != 0 ||
                                 (reinterpret_cast<uintptr_t>(it.ep.resid) & 15) != 0 || it.ep.ldr % 8 != 0))
     return TP_ERR_INVALID_ARGUMENT;
@@ -247,7 +248,19 @@ int make_one_cta_maps(const GemmItem& it, int block_n, CUtensorMap* map_a, CUten
 // The CLIP tower's epilogue features (residual add, quick_gelu) run in instantiations of their own (tp_gemm.cuh: kTower)
 bool tower_epilogue(const GemmEpilogue& ep) { return ep.resid != nullptr || ep.gelu == 2; }   // (an fp32 output alone stays on the projector's)
 
-template <int kBlockN, bool kTower>
+// The instantiation that runs an item: 0 the projector's, 1 the bf16 tower's (inferred from the epilogue features, so that a bf16 tower's
+// plain items — patch embedding, qkv — run on the projector's), 2 the f16 tower's (selected by GemmEpilogue::f16 alone: every f16 item,
+// plain ones included, runs there)
+int gemm_variant(const GemmEpilogue& ep) { return ep.f16 ? 2 : tower_epilogue(ep) ? 1 : 0; }
+
+// One launch runs one instantiation, and a chain's stages hand 16-bit data from one to the next: f16 and bf16 items never share either
+bool mixed_precision(const GemmItem* items, int count) {
+  for (int i = 1; i < count; ++i)
+    if (items[i].ep.f16 != items[0].ep.f16) return true;
+  return false;
+}
+
+template <int kBlockN, bool kTower, bool kF16 = false>
 int launch_gemm_tt(const GemmItem& it, const CUtensorMap& map_a, const CUtensorMap& map_b, int sms, cudaStream_t stream) {
   using Cfg = GemmConfig<kBlockN>;
   {
@@ -255,22 +268,25 @@ int launch_gemm_tt(const GemmItem& it, const CUtensorMap& map_a, const CUtensorM
     int dev = 0;
     TP_CUDA(cudaGetDevice(&dev));
     if (dev >= 32 || !(attr_done & (1u << dev))) {
-      TP_CUDA(cudaFuncSetAttribute(tp_gemm_kernel<kBlockN, kTower>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+      TP_CUDA(cudaFuncSetAttribute(tp_gemm_kernel<kBlockN, kTower, kF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
       if (dev < 32) attr_done |= 1u << dev;
     }
   }
   const long long tiles = ((it.M + kBlockM - 1) / kBlockM) * ((it.N + kBlockN - 1) / kBlockN);
   const int grid = static_cast<int>(tiles < sms ? tiles : sms);
   GemmEpilogue ep = it.ep;
-  TP_CUDA(launch_pdl(tp_gemm_kernel<kBlockN, kTower>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, map_a, map_b,
+  TP_CUDA(launch_pdl(tp_gemm_kernel<kBlockN, kTower, kF16>, dim3(grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, map_a, map_b,
                      static_cast<int>(it.M), static_cast<int>(it.N), static_cast<int>(it.K), static_cast<int>(it.a.seg_rows), ep));
   return TP_OK;
 }
 
 template <int kBlockN>
 int launch_gemm_t(const GemmItem& it, const CUtensorMap& map_a, const CUtensorMap& map_b, int sms, cudaStream_t stream) {
-  return tower_epilogue(it.ep) ? launch_gemm_tt<kBlockN, true>(it, map_a, map_b, sms, stream)
-                               : launch_gemm_tt<kBlockN, false>(it, map_a, map_b, sms, stream);
+  switch (gemm_variant(it.ep)) {
+    case 2: return launch_gemm_tt<kBlockN, true, true>(it, map_a, map_b, sms, stream);
+    case 1: return launch_gemm_tt<kBlockN, true>(it, map_a, map_b, sms, stream);
+    default: return launch_gemm_tt<kBlockN, false>(it, map_a, map_b, sms, stream);
+  }
 }
 
 // Everything a launch of the pair kernel needs, as built from a list of items: kept by the forward plan cache below (encoding
@@ -287,10 +303,10 @@ int build_pair_group(const GemmItem* items, int count, int sms, const FrontWork*
   GemmGroup& g = out->g;
   memset(&g, 0, sizeof(g));
   g.count = count;
-  // one launch runs one instantiation (launch_built): tower epilogues and the projector's features never share a group
+  // one launch runs one instantiation (launch_built): tower epilogues and the projector's features, f16 and bf16 items never share a group
   for (int i = 1; i < count; ++i)
-    if (tower_epilogue(items[i].ep) != tower_epilogue(items[0].ep)) return TP_ERR_INVALID_ARGUMENT;
-  if (count > 0 && tower_epilogue(items[0].ep) && front != nullptr) return TP_ERR_INVALID_ARGUMENT;   // no front work there either
+    if (gemm_variant(items[i].ep) != gemm_variant(items[0].ep)) return TP_ERR_INVALID_ARGUMENT;
+  if (count > 0 && gemm_variant(items[0].ep) != 0 && front != nullptr) return TP_ERR_INVALID_ARGUMENT;   // no front work there either
   long long total = 0;
   for (int i = 0; i < count; ++i) {
     const GemmItem& it = items[i];
@@ -501,7 +517,7 @@ int build_pair_group(const GemmItem* items, int count, int sms, const FrontWork*
   return TP_OK;
 }
 
-template <bool kTower>
+template <bool kTower, bool kF16 = false>
 int launch_built_t(const BuiltLaunch& b, cudaStream_t stream) {
   using Cfg = Gemm2Config;
   {
@@ -509,18 +525,22 @@ int launch_built_t(const BuiltLaunch& b, cudaStream_t stream) {
     int dev = 0;
     TP_CUDA(cudaGetDevice(&dev));
     if (dev >= 32 || !(attr_done & (1u << dev))) {
-      TP_CUDA(cudaFuncSetAttribute(tp_gemm2_kernel<kTower>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+      TP_CUDA(cudaFuncSetAttribute(tp_gemm2_kernel<kTower, kF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
       if (dev < 32) attr_done |= 1u << dev;
     }
   }
-  TP_CUDA(launch_pdl(tp_gemm2_kernel<kTower>, dim3(b.grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, b.g, b.peers));
+  TP_CUDA(launch_pdl(tp_gemm2_kernel<kTower, kF16>, dim3(b.grid), dim3(kGemmThreads), Cfg::kSmemBytes, stream, b.g, b.peers));
   return TP_OK;
 }
 
 int launch_built(const BuiltLaunch& b, cudaStream_t stream) {
-  bool tower = false;
-  for (int i = 0; i < b.g.count; ++i) tower = tower || tower_epilogue(b.g.p[i].ep);
-  return tower ? launch_built_t<true>(b, stream) : launch_built_t<false>(b, stream);
+  int variant = 0;                                     // the same for every problem (build_pair_group)
+  for (int i = 0; i < b.g.count; ++i) variant = gemm_variant(b.g.p[i].ep) > variant ? gemm_variant(b.g.p[i].ep) : variant;
+  switch (variant) {
+    case 2: return launch_built_t<true, true>(b, stream);
+    case 1: return launch_built_t<true>(b, stream);
+    default: return launch_built_t<false>(b, stream);
+  }
 }
 
 // Build and launch; built != nullptr: the launch is kept there for replay (the forward plan cache)
@@ -581,7 +601,7 @@ int gemm_mode() {
 }
 
 int launch_gemms(const GemmItem* items, int count, int sms, cudaStream_t stream) {
-  if (count <= 0 || count > kMaxGroup) return TP_ERR_INVALID_ARGUMENT;
+  if (count <= 0 || count > kMaxGroup || mixed_precision(items, count)) return TP_ERR_INVALID_ARGUMENT;
   const int mode = gemm_mode();
   // Every item is checked, placed and encoded before the first launch: an invalid item anywhere in the list launches nothing.
   int choice[kMaxGroup];
@@ -647,7 +667,7 @@ bool chain_feasible(const GemmItem* items, int count, int sms, bool by_cost = tr
 
 int launch_chain(GemmItem* items, int count, int* flags, long long flag_capacity, const FrontWork* front, int sms, cudaStream_t stream,
                  BuiltLaunch* built = nullptr) {
-  if (count <= 0 || count > kMaxGroup) return TP_ERR_INVALID_ARGUMENT;
+  if (count <= 0 || count > kMaxGroup || mixed_precision(items, count)) return TP_ERR_INVALID_ARGUMENT;
   for (int i = 0; i < count; ++i) {
     const int deps[3] = {items[i].dep, items[i].dep2, items[i].dep3};
     for (int d : deps) {

@@ -3,7 +3,10 @@
 //   clip_embed_preln_kernel    + class / position embedding, pre_layrnorm -> hidden_states[0]
 //   clip_layernorm_kernel      layer_norm1 / layer_norm2 of a layer
 //   clip_attn_kernel           softmax(q k^T) v per (crop, head, 128-query block) over the 577 tokens, wgmma + online softmax
+// Each is instantiated for the bf16 tower and for the fp16 one (__half storage, f16 wgmma); the arithmetic is fp32 in both.
 #pragma once
+
+#include <type_traits>
 
 #include "tp_ptx.cuh"
 
@@ -18,9 +21,10 @@ constexpr int kClipHeads = 16;
 constexpr int kClipHeadDim = 64;
 constexpr float kClipLnEps = 1e-5f;
 
-// One thread per (patch row, channel, kernel row): 14 consecutive pixels in, 14 consecutive patch-row elements out.
-__global__ void clip_im2col_kernel(const __nv_bfloat16* __restrict__ crops, long long crop_stride, long long n_crops,
-                                   __nv_bfloat16* __restrict__ patches) {
+// One thread per (patch row, channel, kernel row): 14 consecutive pixels in, 14 consecutive patch-row elements out.  bf16 crops into
+// f16 patch rows are converted as images.to(torch.float16) does (clip_encoder.py:59): through fp32, one round-to-nearest-even.
+template <typename Tin, typename Tout>
+__global__ void clip_im2col_kernel(const Tin* __restrict__ crops, long long crop_stride, long long n_crops, Tout* __restrict__ patches) {
   const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (idx >= n_crops * 576 * 3 * kClipPatch) return;
   const int cy = static_cast<int>(idx % (3 * kClipPatch));
@@ -29,16 +33,21 @@ __global__ void clip_im2col_kernel(const __nv_bfloat16* __restrict__ crops, long
   const int p = static_cast<int>(prow - n * 576);
   const int c = cy / kClipPatch, ky = cy - c * kClipPatch;
   const int py = p / 24, px = p - py * 24;
-  const __nv_bfloat16* src = crops + n * crop_stride + (static_cast<long long>(c) * kClipImage + py * kClipPatch + ky) * kClipImage + px * kClipPatch;
-  __nv_bfloat16* dst = patches + prow * kClipPatchLd + cy * kClipPatch;
+  const Tin* src = crops + n * crop_stride + (static_cast<long long>(c) * kClipImage + py * kClipPatch + ky) * kClipImage + px * kClipPatch;
+  Tout* dst = patches + prow * kClipPatchLd + cy * kClipPatch;
 #pragma unroll
-  for (int kx = 0; kx < kClipPatch; ++kx) dst[kx] = src[kx];
+  for (int kx = 0; kx < kClipPatch; ++kx) {
+    if constexpr (std::is_same_v<Tin, Tout>) dst[kx] = src[kx];
+    else dst[kx] = __float2half_rn(__bfloat162float(src[kx]));
+  }
 }
 
-// LayerNorm of one 1024-wide row held by a warp in fp32 (lane l: columns 256 j + 8 l + [0, 8), j = 0..3), one rounding to bf16:
-// mean, then the variance from the deviations (two passes over registers), rstd = rsqrt(var + 1e-5)
-__device__ __forceinline__ void clip_ln_row_store(const float (&e)[32], const __nv_bfloat16* __restrict__ gamma,
-                                                  const __nv_bfloat16* __restrict__ beta, __nv_bfloat16* __restrict__ out, int lane) {
+// LayerNorm of one 1024-wide row held by a warp in fp32 (lane l: columns 256 j + 8 l + [0, 8), j = 0..3), one rounding to T (bf16 or
+// f16, the type of gamma and beta too): mean, then the variance from the deviations (two passes over registers), rstd = rsqrt(var + 1e-5)
+template <typename T>
+__device__ __forceinline__ void clip_ln_row_store(const float (&e)[32], const T* __restrict__ gamma, const T* __restrict__ beta,
+                                                  T* __restrict__ out, int lane) {
+  constexpr bool kF16 = std::is_same_v<T, __half>;
   float s = 0.f;
 #pragma unroll
   for (int i = 0; i < 32; ++i) s += e[i];
@@ -62,8 +71,8 @@ __device__ __forceinline__ void clip_ln_row_store(const float (&e)[32], const __
     uint32_t o[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k)
-      o[k] = pack_bf16x2(fmaf((e[8 * j + 2 * k] - mean) * rstd, bf16_lo(gw[k]), bf16_lo(bw[k])),
-                         fmaf((e[8 * j + 2 * k + 1] - mean) * rstd, bf16_hi(gw[k]), bf16_hi(bw[k])));
+      o[k] = pack_x2<kF16>(fmaf((e[8 * j + 2 * k] - mean) * rstd, x2_lo<kF16>(gw[k]), x2_lo<kF16>(bw[k])),
+                           fmaf((e[8 * j + 2 * k + 1] - mean) * rstd, x2_hi<kF16>(gw[k]), x2_hi<kF16>(bw[k])));
     *reinterpret_cast<uint4*>(out + col) = make_uint4(o[0], o[1], o[2], o[3]);
   }
 }
@@ -91,11 +100,24 @@ __device__ __forceinline__ void clip_load_row(const __nv_bfloat16* __restrict__ 
   }
 }
 
+__device__ __forceinline__ void clip_load_row(const __half* __restrict__ src, float (&e)[32], int lane) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const uint4 a = *reinterpret_cast<const uint4*>(src + 256 * j + 8 * lane);
+    const uint32_t aw[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      e[8 * j + 2 * k] = f16_lo(aw[k]);
+      e[8 * j + 2 * k + 1] = f16_hi(aw[k]);
+    }
+  }
+}
+
 // One warp per token row of x ([N*577, 1024], rows n*577 + t; rows t >= 1 hold the patch embedding, row 0 is ignored):
-//   x[row] = bf16(pre_layrnorm((t == 0 ? class_embedding : x[row]) + position_embedding[t]))    (fp32 sum, in place, one rounding)
-__global__ void clip_embed_preln_kernel(__nv_bfloat16* __restrict__ x, long long rows, const __nv_bfloat16* __restrict__ cls,
-                                        const __nv_bfloat16* __restrict__ pos, const __nv_bfloat16* __restrict__ gamma,
-                                        const __nv_bfloat16* __restrict__ beta) {
+//   x[row] = T(pre_layrnorm((t == 0 ? class_embedding : x[row]) + position_embedding[t]))    (fp32 sum, in place, one rounding)
+template <typename T>
+__global__ void clip_embed_preln_kernel(T* __restrict__ x, long long rows, const T* __restrict__ cls, const T* __restrict__ pos,
+                                        const T* __restrict__ gamma, const T* __restrict__ beta) {
   const long long row = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
@@ -108,12 +130,12 @@ __global__ void clip_embed_preln_kernel(__nv_bfloat16* __restrict__ x, long long
   clip_ln_row_store(e, gamma, beta, x + row * 1024, lane);
 }
 
-// y = bf16(LayerNorm(x) * gamma + beta), one warp per row of [rows, 1024]: layer_norm1 (x: the bf16 hidden state) / layer_norm2 (x: the
-// fp32 mid-layer residual) of a layer, as an explicit pass (statistics from the row itself, in fp32) so that the following linear reads
-// its weights as they are
-template <typename T>
-__global__ void clip_layernorm_kernel(const T* __restrict__ x, long long rows, const __nv_bfloat16* __restrict__ gamma,
-                                      const __nv_bfloat16* __restrict__ beta, __nv_bfloat16* __restrict__ y) {
+// y = Tp(LayerNorm(x) * gamma + beta), one warp per row of [rows, 1024]: layer_norm1 (x: the bf16 / f16 hidden state) / layer_norm2 (x:
+// the fp32 mid-layer residual) of a layer, as an explicit pass (statistics from the row itself, in fp32) so that the following linear
+// reads its weights as they are.  Tp: the tower's storage type (gamma, beta and y).
+template <typename T, typename Tp = __nv_bfloat16>
+__global__ void clip_layernorm_kernel(const T* __restrict__ x, long long rows, const Tp* __restrict__ gamma, const Tp* __restrict__ beta,
+                                      Tp* __restrict__ y) {
   const long long row = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
@@ -124,8 +146,10 @@ __global__ void clip_layernorm_kernel(const T* __restrict__ x, long long rows, c
 
 // ------------------------------------------------------------------------------------------------
 // Attention over the 577 tokens of one crop, one head, 128 queries (two warpgroups of 64):
-//   qkv  [N*577, 3072] bf16: q (already scaled by 1/8 in the packed weights) | k | v, head h at columns 64 h of each third
-//   ctx  [N*577, 1024] bf16: heads side by side (HF's reshape of [N, 577, 16, 64])
+//   qkv  [N*577, 3072] T: q (already scaled by 1/8: in the packed bf16 weights, by the q GEMM's alpha in f16) | k | v, head h at columns
+//        64 h of each third
+//   ctx  [N*577, 1024] T: heads side by side (HF's reshape of [N, 577, 16, 64])
+// T = bf16 or f16: the wgmmas take T operands, P is rounded to T.
 // Thread 0 loads the CTA's Q rows and the whole K and V of the (crop, head) by TMA through a 3-D (column, token, crop) map whose
 // token extent is 577: boxes reaching past token 576 are zero-filled, never the next crop's rows.  Per 128-key block:
 //   S = Q K^T (wgmma m64n128k16, both K-major), keys >= 577 set to -inf BEFORE the row max (a zero-filled key scores 0 and would take
@@ -144,8 +168,10 @@ struct ClipAttnSmem {
 };
 static_assert(ClipAttnSmem::kBytes <= 232448, "shared memory budget of an sm_90 SM (227 KiB)");
 
+template <typename T>
 __global__ void __launch_bounds__(256, 1)
-clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, __nv_bfloat16* __restrict__ ctx) {
+clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, T* __restrict__ ctx) {
+  constexpr bool kF16 = std::is_same_v<T, __half>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem + ClipAttnSmem::kBar);
@@ -186,7 +212,7 @@ clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, __nv_bfloat16* __
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < kClipHeadDim / kUmmaK; ++k)
-      wgmma_m64n128<0, 0>(s, make_smem_desc_kmajor_sw128(sq) + static_cast<uint64_t>(k * 2),
+      wgmma_m64n128<0, 0, kF16>(s, make_smem_desc_kmajor_sw128(sq) + static_cast<uint64_t>(k * 2),
                           make_smem_desc_kmajor_sw128(sk + kb * 2 * kAttnBoxBytes) + static_cast<uint64_t>(k * 2), static_cast<uint32_t>(k != 0));
     wgmma_commit();
     wgmma_wait<0>();
@@ -211,7 +237,7 @@ clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, __nv_bfloat16* __
     }
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] *= corr[(i >> 1) & 1];
-    // P = exp2((s - m) log2 e), rounded to bf16; the rounded values are summed and stored (K-major, 128-byte swizzle: row r's 16-byte
+    // P = exp2((s - m) log2 e), rounded to T; the rounded values are summed and stored (K-major, 128-byte swizzle: row r's 16-byte
     // chunk c of a 64-key half lies at r * 128 + ((c ^ (r & 7)) << 4))
     const float nm0 = -m[0] * kLog2e, nm1 = -m[1] * kLog2e;
     named_bar_sync(1 + wg, 128);                           // the previous block's P V wgmmas of the whole warpgroup have retired
@@ -219,8 +245,8 @@ clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, __nv_bfloat16* __
     for (int i = 0; i < 64; i += 2) {
       const int h = (i >> 1) & 1;
       const float nm = h ? nm1 : nm0;
-      const uint32_t pk = pack_bf16x2(ex2_approx(fmaf(s[i], kLog2e, nm)), ex2_approx(fmaf(s[i + 1], kLog2e, nm)));
-      l[h] += bf16_lo(pk) + bf16_hi(pk);
+      const uint32_t pk = pack_x2<kF16>(ex2_approx(fmaf(s[i], kLog2e, nm)), ex2_approx(fmaf(s[i + 1], kLog2e, nm)));
+      l[h] += x2_lo<kF16>(pk) + x2_hi<kF16>(pk);
       const int r = 16 * warp + g + 8 * h;
       const int col = 8 * (i >> 2) + 2 * q;
       const int half = col >> 6, c64 = col & 63;
@@ -233,7 +259,7 @@ clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, __nv_bfloat16* __
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 128 / kUmmaK; ++k)
-      wgmma_m64n64<0, 1>(o, make_smem_desc_kmajor_sw128(sp + (k >> 2) * kAttnBoxBytes) + static_cast<uint64_t>((k & 3) * 2),
+      wgmma_m64n64<0, 1, kF16>(o, make_smem_desc_kmajor_sw128(sp + (k >> 2) * kAttnBoxBytes) + static_cast<uint64_t>((k & 3) * 2),
                          make_smem_desc_mnmajor_sw128(sv + (kb * 2 + (k >> 2)) * kAttnBoxBytes, kAttnBoxBytes) + static_cast<uint64_t>((k & 3) * 128),
                          1u);
     wgmma_commit();
@@ -251,14 +277,15 @@ clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, __nv_bfloat16* __
   for (int h = 0; h < 2; ++h) {
     const int t = qb * 128 + wg * 64 + 16 * warp + g + 8 * h;
     if (t >= kClipTokens) continue;
-    __nv_bfloat16* dst = ctx + (static_cast<long long>(crop) * kClipTokens + t) * 1024 + head * kClipHeadDim + 2 * q;
+    T* dst = ctx + (static_cast<long long>(crop) * kClipTokens + t) * 1024 + head * kClipHeadDim + 2 * q;
 #pragma unroll
     for (int i = 2 * h; i < 32; i += 4)
-      *reinterpret_cast<uint32_t*>(dst + 8 * (i >> 2)) = pack_bf16x2(__fmul_rn(o[i], inv[h]), __fmul_rn(o[i + 1], inv[h]));
+      *reinterpret_cast<uint32_t*>(dst + 8 * (i >> 2)) = pack_x2<kF16>(__fmul_rn(o[i], inv[h]), __fmul_rn(o[i + 1], inv[h]));
   }
 }
 
-// The q third of the packed [3072, 1024] qkv weight and its fp32 bias times 1/8 (exact: a power of two)
+// The q third of the packed [3072, 1024] qkv weight and its fp32 bias times 1/8 (exact: a power of two in bf16, whose exponent range is
+// fp32's; the f16 tower applies 1/8 as the q GEMM's alpha instead, since weights below 2^-11 would lose bits as f16 subnormals)
 __global__ void clip_scale_q_kernel(__nv_bfloat16* __restrict__ w, float* __restrict__ bias) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < 1024 * 1024) w[i] = __float2bfloat16_rn(__bfloat162float(w[i]) * 0.125f);

@@ -1,6 +1,7 @@
 // Persistent warp-specialised wgmma GEMMs for sm_90a with the fused epilogues the TokenPacker path needs.
 //
 //   C[M,N] (bf16) = epilogue( A[M,K] (bf16, K-major) . B[N,K]^T (bf16, K-major) ),  fp32 accumulation in registers.
+//   (The CLIP tower's fp16 instantiations, kF16: the same with f16 operands and output, GemmEpilogue::f16.)
 //
 // Every nn.Linear on the reference hot path (builder.py:59-83; MHA in/out projections builder.py:77) is an
 // instance of these kernels: activations are [rows, in] and weights are [out, in], both K-major, which is exactly the
@@ -43,7 +44,7 @@
 namespace tp {
 
 struct GemmEpilogue {
-  __nv_bfloat16* c;        // output
+  void* c;                 // output: bf16 [M, ldc] (f16 with f16, float with out_f32)
   long long ldc;           // elements between output rows
   const float* col_a;      // [N]  LN fold: row-sum of the gamma-folded weight      (nullptr: no LN fold)
   const float* col_b;      // [N]  bias                                             (nullptr: none)
@@ -68,10 +69,14 @@ struct GemmEpilogue {
   int dual;                // 1 (with gelu): the bf16-rounded PRE-activation (after bias / LN fold, before GELU and alpha) is stored too,
                            // through GemmProblem::tmap_cx[0] (the training forward keeps z for GELU'(z); builder.py:66-75 under autograd).
                            // Pair kernel, plain (unsegmented) TMA-store output, two 64-column staging buffers per half.
-  const __nv_bfloat16* resid;   // != nullptr: v += resid[row * ldr + c] after bias / LN fold (the CLIP tower's residual stream), read
-  long long ldr;                // straight from global memory (the pair kernel's shared memory is full); row = the GEMM row
+  const void* resid;            // != nullptr: v += resid[row * ldr + c] after bias / LN fold (the CLIP tower's residual stream), read
+  long long ldr;                // straight from global memory (the pair kernel's shared memory is full); row = the GEMM row; bf16
+                                // values (f16 with f16)
   int resid_f32;                // 1: resid points to float values (the tower's unrounded mid-layer residual x')
+  int f16;                      // 1: A, B, C and a 16-bit resid are IEEE half: the tower's f16 instantiations run the item (kF16)
 };
+// f16 fills the padding after resid_f32: every other field keeps its offset, so the kernels' parameter blocks are laid out as before
+static_assert(sizeof(GemmEpilogue) == 128 && offsetof(GemmEpilogue, f16) == 124, "GemmEpilogue layout");
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;     // 64 bf16 = 128 bytes = one swizzle-128B row
@@ -135,7 +140,7 @@ __device__ __forceinline__ void acc_chunk(const float (&acc)[2][kAccN], int chun
 // One warpgroup's MMAs for a tile: the CTA's 128 rows of A (two 64-row blocks) x kN columns of B starting `b_off` bytes into
 // the stage's B tile, over n_kb k-blocks of the ring.  A stage is released (one arrive per warp on empty_bar) once the wgmmas
 // reading it have retired; one k-block of wgmmas stays in flight while the next one is issued.
-template <int kN, int kTransA, int kTransB>
+template <int kN, int kTransA, int kTransB, bool kF16 = false>
 __device__ __forceinline__ void mma_tile(float (&acc)[2][kN / 2], const uint8_t* smem, int stage_bytes, int a_bytes, int b_off,
                                          uint64_t* full_bar, uint64_t* empty_bar, int n_stages, int& stage, uint32_t& phase, int n_kb) {
   static_assert(kN == 64 || kN == 128, "wgmma N");
@@ -159,8 +164,8 @@ __device__ __forceinline__ void mma_tile(float (&acc)[2][kN / 2], const uint8_t*
         const uint32_t sam = sa + static_cast<uint32_t>(mb * 8192);
         const uint64_t da = kTransA ? make_smem_desc_mnmajor_sw128(sam, 8192) + static_cast<uint64_t>(k * 128)
                                     : make_smem_desc_kmajor_sw128(sam) + static_cast<uint64_t>(k * 2);
-        if constexpr (kN == 128) wgmma_m64n128<kTransA, kTransB>(acc[mb], da, db, accumulate);
-        else wgmma_m64n64<kTransA, kTransB>(acc[mb], da, db, accumulate);
+        if constexpr (kN == 128) wgmma_m64n128<kTransA, kTransB, kF16>(acc[mb], da, db, accumulate);
+        else wgmma_m64n64<kTransA, kTransB, kF16>(acc[mb], da, db, accumulate);
       }
     }
     wgmma_commit();
@@ -246,7 +251,8 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
 
 // kTower: the CLIP tower's instantiations (bias, bf16 or fp32 residual add, quick_gelu, alpha, fp32 output) — and none of the
 // projector's LayerNorm fold, row statistics, dual / window-major outputs, so that neither set of instantiations carries the other's registers.
-template <int kTileN, bool kTower = false>
+// kF16 (tower only): the same with an f16 residual and f16 output (one __floats2half2_rn rounding).
+template <int kTileN, bool kTower = false, bool kF16 = false>
 __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int N, const float (&acc)[2][kTileN / 4], uint32_t scratch,
                                               int row, int col_tile0, int quarter, int half, const float* s_col, const OutStage& out,
                                               long long c_extra = 0) {
@@ -268,7 +274,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
     const int seg = row / ep.seg_len;
     dst_row = static_cast<long long>(seg) * ep.seg_stride + (row - seg * ep.seg_len);
   }
-  __nv_bfloat16* c_row = ep.c + dst_row * ep.ldc;
+  __nv_bfloat16* c_row = static_cast<__nv_bfloat16*>(ep.c) + dst_row * ep.ldc;     // 16-bit elements (bf16 or f16: stored as raw bits)
   float* c_row32 = reinterpret_cast<float*>(ep.c) + c_extra + dst_row * ep.ldc;     // out_f32 only (c_extra: split-K slice)
   const uint32_t sa_addr = smem_u32(s_col + half * kColsPerWarp), sb_addr = smem_u32(s_col + kTileN + half * kColsPerWarp);
   const uint32_t out_addr = out.buf != nullptr ? smem_u32(out.buf) : 0u;
@@ -347,15 +353,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
               v[2 * g] = add2(v[2 * g], pk2(r4.x, r4.y));
               v[2 * g + 1] = add2(v[2 * g + 1], pk2(r4.z, r4.w));
             }
-          } else if (ep.resid != nullptr && row_ok) {   // one bf16 rounding of acc + bias + R: the residual add of a CLIP layer
-            const uint4* rp = reinterpret_cast<const uint4*>(ep.resid + static_cast<long long>(row) * ep.ldr + col0 + sub * kSubPairs * 2);
+          } else if (ep.resid != nullptr && row_ok) {   // one rounding of acc + bias + R: the residual add of a CLIP layer
+            const uint4* rp = reinterpret_cast<const uint4*>(static_cast<const __nv_bfloat16*>(ep.resid) + static_cast<long long>(row) * ep.ldr +
+                                                             col0 + sub * kSubPairs * 2);
 #pragma unroll
             for (int g = 0; g < kSubPairs / 4; ++g) {
               const uint4 r4 = rp[g];
-              v[4 * g] = add2(v[4 * g], pk2(bf16_lo(r4.x), bf16_hi(r4.x)));
-              v[4 * g + 1] = add2(v[4 * g + 1], pk2(bf16_lo(r4.y), bf16_hi(r4.y)));
-              v[4 * g + 2] = add2(v[4 * g + 2], pk2(bf16_lo(r4.z), bf16_hi(r4.z)));
-              v[4 * g + 3] = add2(v[4 * g + 3], pk2(bf16_lo(r4.w), bf16_hi(r4.w)));
+              v[4 * g] = add2(v[4 * g], pk2(x2_lo<kF16>(r4.x), x2_hi<kF16>(r4.x)));
+              v[4 * g + 1] = add2(v[4 * g + 1], pk2(x2_lo<kF16>(r4.y), x2_hi<kF16>(r4.y)));
+              v[4 * g + 2] = add2(v[4 * g + 2], pk2(x2_lo<kF16>(r4.z), x2_hi<kF16>(r4.z)));
+              v[4 * g + 3] = add2(v[4 * g + 3], pk2(x2_lo<kF16>(r4.w), x2_hi<kF16>(r4.w)));
             }
           }
           if (ep.gelu == 2) {
@@ -375,7 +382,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
         for (int j = 0; j < kSubPairs; ++j) {
           float lo, hi;
           upk2(v[j], lo, hi);
-          pk[j] = pack_bf16x2(lo, hi);
+          pk[j] = pack_x2<kF16>(lo, hi);
         }
         if (do_stats) {    // LayerNorm statistics of the ROUNDED values the next GEMM will read (column order: deterministic)
           if (chunk == 0 && sub == 0) shift = bf16_lo(pk[0]);
@@ -587,7 +594,7 @@ struct GemmConfig {
   static_assert(kSmemBytes <= 232448, "shared memory budget of an sm_90 SM (227 KiB)");
 };
 
-template <int kBlockN, bool kTower = false>
+template <int kBlockN, bool kTower = false, bool kF16 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, int M, int N, int K,
                int a_seg_rows, GemmEpilogue ep) {
@@ -595,6 +602,7 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   constexpr int kStages = Cfg::kStages;
   constexpr int kN = kBlockN / 2;                  // columns per warpgroup
   static_assert(kBlockN == 128 || kBlockN == 256, "BLOCK_N");
+  static_assert(kTower || !kF16, "f16 instantiations are the tower's");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -670,10 +678,10 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       const int m_blk = tile / num_n_blocks;
       const int n_blk = tile - m_blk * num_n_blocks;
       stage_col_vectors<kBlockN>(ep, N, n_blk * kBlockN, s_col, epi_tid, true);
-      mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, half * kN * kBlockK * 2, full_bar, empty_bar, kStages, stage, phase,
-                         num_k_blocks);
+      mma_tile<kN, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, half * kN * kBlockK * 2, full_bar, empty_bar, kStages, stage, phase,
+                               num_k_blocks);
       const OutStage no_stage{nullptr, nullptr, nullptr, 0u};
-      epilogue_tile<kBlockN, kTower>(ep, M, N, acc, scratch, m_blk * kBlockM + epi_row(quarter, lane), n_blk * kBlockN, quarter, half, s_col,
+      epilogue_tile<kBlockN, kTower, kF16>(ep, M, N, acc, scratch, m_blk * kBlockM + epi_row(quarter, lane), n_blk * kBlockN, quarter, half, s_col,
                                      no_stage);
     }
   }
@@ -807,9 +815,10 @@ __device__ __forceinline__ TileRef decode_tile(const GemmGroup& g, int tile) {
   return t;
 }
 
-template <bool kTower = false>
+template <bool kTower = false, bool kF16 = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ PeerStores peers) {
+  static_assert(kTower || !kF16, "f16 instantiations are the tower's");
   using Cfg = Gemm2Config;
   constexpr int kStages = Cfg::kStages;
   constexpr int kTileN = Cfg::kTileN;
@@ -942,11 +951,11 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       else if (!kTower && pr.ab_mn_major == 2)
         mma_tile<kN, 0, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
       else
-        mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
+        mma_tile<kN, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
       const OutStage out{pr.use_tma_store ? s_out + half * Cfg::kOutBufs * kOutSlabBytes : nullptr, slab_full_bar + half * Cfg::kOutBufs,
                          slab_empty_bar + half * Cfg::kOutBufs, slab_seq};
       if (pr.use_tma_store) slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);     // slabs per tile and column half
-      epilogue_tile<kTileN, kTower>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, quarter, half, s_col, out,
+      epilogue_tile<kTileN, kTower, kF16>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, quarter, half, s_col, out,
                                     static_cast<long long>(t.split) * pr.c_split_stride);
     }
   } else {

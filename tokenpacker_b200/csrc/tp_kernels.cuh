@@ -235,6 +235,12 @@ __global__ void bf16_to_f32_multi_kernel(CastSegs segs) {
   const CastSeg g = segs.s[blockIdx.y];
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < g.n; i += gridDim.x * blockDim.x) g.dst[i] = __bfloat162float(g.src[i]);
 }
+// The same for segments whose src holds IEEE half values (the fp16 CLIP tower's biases)
+__global__ void f16_to_f32_multi_kernel(CastSegs segs) {
+  const CastSeg g = segs.s[blockIdx.y];
+  const __half* src = reinterpret_cast<const __half*>(g.src);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < g.n; i += gridDim.x * blockDim.x) g.dst[i] = __half2float(src[i]);
+}
 
 // LayerNorm folded into the following linear (one warp per output feature o):
 //   LN(y) W^T + b = rstd * ( y (gamma.W)^T - mu * rowsum(gamma.W) ) + ( W beta + b )

@@ -8,6 +8,10 @@ and without keeping the other 21 hidden states alive.  The reference's ``encode_
 
 transformers is never imported: any module with CLIPVisionModel's parameter names (with or without the ``vision_model.`` prefix)
 and a ``.config`` carrying its fields is accepted.
+
+``CLIPVisionTowerB200(model, dtype=torch.float16)`` runs the tower in fp16, as the reference's evaluation and serving scripts do
+(``vision_tower.to(dtype=torch.float16)``, llava/eval/model_vqa_loader.py): the hidden states come back fp16, and the caller casts them
+to bf16 for the projector as clip_encoder.py does (``[h.to(torch.bfloat16) for h in hs]``).
 """
 from __future__ import annotations
 
@@ -45,13 +49,17 @@ def _check_config(cfg):
 class CLIPVisionTowerB200(nn.Module):
     """Forward-only CLIPVisionModel (openai/clip-vit-large-patch14-336) up to hidden_states[23].
 
+    dtype: the precision the tower computes in.  None (the default) or torch.bfloat16: bf16 storage, and fp16 / fp32 towers are cast
+    to bf16 once, with a warning.  torch.float16: fp16 storage (fp16 parameters read in place, others cast to fp16 once), fp16 outputs.
     The wrapped model stays the owner of the parameters (``self.vision_model``).  A derived cache (about 147 MB: per layer the q/k/v
-    concatenation with q scaled by 1/8, and the biases in fp32) is keyed on every parameter's ``(data_ptr, _version, dtype)``
-    and dropped by ``load_state_dict``, ``.to()`` / ``.cuda()`` / ``.half()`` and ``invalidate_packed()``.  fp16 / fp32 towers are cast
-    to bf16 once, with a warning."""
+    concatenation — with q scaled by 1/8 in bf16 —, and the biases in fp32) is keyed on the compute precision and every parameter's
+    ``(data_ptr, _version, dtype)``, and dropped by ``load_state_dict``, ``.to()`` / ``.cuda()`` / ``.half()`` and
+    ``invalidate_packed()``."""
 
-    def __init__(self, vision_model: nn.Module):
+    def __init__(self, vision_model: nn.Module, dtype: torch.dtype | None = None):
         super().__init__()
+        if dtype not in (None, torch.bfloat16, torch.float16):
+            raise ValueError(f"CLIPVisionTowerB200 computes in torch.bfloat16 (dtype=None) or torch.float16, not {dtype!r}")
         _check_config(getattr(vision_model, "config", None))
         named = dict(vision_model.named_parameters())
         prefix = "vision_model." if "vision_model.embeddings.class_embedding" in named else ""
@@ -62,6 +70,7 @@ class CLIPVisionTowerB200(nn.Module):
         if missing:
             raise NotImplementedError(f"not a CLIPVisionModel: parameters {missing[:3]} are missing")
         self.vision_model = vision_model
+        self.dtype = torch.float16 if dtype == torch.float16 else torch.bfloat16
         self._names = names
         self._packed = None
         self._packed_key = None
@@ -86,15 +95,17 @@ class CLIPVisionTowerB200(nn.Module):
 
     def _packed_weights(self, device):
         params = self._params()
-        key = (str(device),) + tuple((p.data_ptr(), p._version, p.dtype) for p in params)
+        key = (str(device), self.dtype) + tuple((p.data_ptr(), p._version, p.dtype) for p in params)
         if self._packed is not None and self._packed_key == key:
             return self._packed, self._weights
-        if any(p.dtype != torch.bfloat16 for p in params) and not self._warned_dtype:
+        f16 = self.dtype == torch.float16
+        if not f16 and any(p.dtype != torch.bfloat16 for p in params) and not self._warned_dtype:
             self._warned_dtype = True
             warnings.warn("CLIPVisionTowerB200 computes with bf16 storage and fp32 accumulation: the tower's fp16 / fp32 parameters are "
                           "cast to bf16 once into the derived cache", UserWarning, stacklevel=3)
-        # bf16 parameters are read in place; anything else (other dtype, non-contiguous, not 16-byte aligned) through a bf16 copy
-        bf = [p.detach().to(device=device, dtype=torch.bfloat16).contiguous() for p in params]
+        # parameters of the compute dtype are read in place; anything else (other dtype, non-contiguous, not 16-byte aligned) through a
+        # copy in it (in fp16 that cast is the reference's own vision_tower.to(dtype=torch.float16): no warning)
+        bf = [p.detach().to(device=device, dtype=self.dtype).contiguous() for p in params]
         bf = [t if t.data_ptr() % 16 == 0 else t.clone() for t in bf]
         n_top = len(_lib.CLIP_TOWER_FIELDS)
         w = _lib.TpClipTowerWeights(*[t.data_ptr() for t in bf[:n_top]])
@@ -104,14 +115,19 @@ class CLIPVisionTowerB200(nn.Module):
         nbytes = lib.tp_clip_tower_packed_bytes()
         packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
         stream = torch.cuda.current_stream(device).cuda_stream
-        check(lib.tp_clip_tower_pack_weights(C.byref(w), packed.data_ptr(), nbytes, stream), "tp_clip_tower_pack_weights")
-        # bf16 parameters are read in place by every forward; the cast copies of other dtypes are kept alive with the cache
+        if f16:
+            check(lib.tp_clip_tower_pack_weights_f16(C.byref(w), packed.data_ptr(), nbytes, stream), "tp_clip_tower_pack_weights_f16")
+        else:
+            check(lib.tp_clip_tower_pack_weights(C.byref(w), packed.data_ptr(), nbytes, stream), "tp_clip_tower_pack_weights")
+        # parameters of the compute dtype are read in place by every forward; the cast copies of others are kept alive with the cache
         self._packed, self._packed_key, self._weights = packed, key, (w, bf)
         return packed, self._weights
 
     def hidden_states(self, images: torch.Tensor):
         """images: [N, 3, 336, 336] CUDA crops (bf16 read in place, any crop stride; other dtypes cast to bf16).  Returns the tuple
-        (hidden_states[12], [16], [22], [23]), each bf16 [N, 577, 1024] with the CLS row."""
+        (hidden_states[12], [16], [22], [23]), each bf16 [N, 577, 1024] with the CLS row.
+        With dtype=torch.float16: bf16 and fp16 crops are read in place (bf16 ones converted as ``images.to(torch.float16)`` rounds
+        them), other dtypes cast to fp16, and the four hidden states are fp16."""
         if not isinstance(images, torch.Tensor) or images.dim() != 4 or tuple(images.shape[1:]) != (3, _IMAGE, _IMAGE):
             shape = tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__
             raise ValueError(f"expected crops [N,3,336,336], got {shape}")
@@ -122,11 +138,12 @@ class CLIPVisionTowerB200(nn.Module):
             raise RuntimeError("tokenpacker_b200 has no CPU path: crops must be CUDA tensors on an H100")
         n = images.shape[0]
         device = images.device
-        outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=torch.bfloat16, device=device) for _ in _OUT_LAYERS)
+        f16 = self.dtype == torch.float16
+        outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=self.dtype, device=device) for _ in _OUT_LAYERS)
         if n == 0:
             return outs
         with torch.cuda.device(device):
-            x = images.to(torch.bfloat16)
+            x = images if f16 and images.dtype in (torch.bfloat16, torch.float16) else images.to(self.dtype)
             if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
                 x = x.contiguous()
             packed, (w, _) = self._packed_weights(device)
@@ -134,6 +151,11 @@ class CLIPVisionTowerB200(nn.Module):
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
             ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
             stream = torch.cuda.current_stream(device).cuda_stream
-            check(lib.tp_clip_tower_forward(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), ptrs, ws.data_ptr(), ws_bytes, stream),
-                  "tp_clip_tower_forward")
+            if f16:
+                crops_dtype = _lib.TP_CLIP_CROPS_F16 if x.dtype == torch.float16 else _lib.TP_CLIP_CROPS_BF16
+                check(lib.tp_clip_tower_forward_f16(packed.data_ptr(), C.byref(w), x.data_ptr(), crops_dtype, n, x.stride(0), ptrs, ws.data_ptr(),
+                                                    ws_bytes, stream), "tp_clip_tower_forward_f16")
+            else:
+                check(lib.tp_clip_tower_forward(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), ptrs, ws.data_ptr(), ws_bytes,
+                                                stream), "tp_clip_tower_forward")
         return outs
