@@ -1,0 +1,418 @@
+"""Training the top of the CLIP tower on the GPU (include/tokenpacker_b200_clip_tower_train.h, CLIPVisionTowerB200(trainable_layers=K)):
+the attention backward, the quick_gelu and LayerNorm backward kernels one by one against fp64 computed from the bf16 operands they
+read; the training forward's outputs bit for bit against the inference forward and its saved set against fp64; every parameter
+gradient of the last K layers against the fp64 autograd oracle; composition with the preprocessing and the projector."""
+import ctypes as C
+import os
+
+import pytest
+import torch
+
+from oracle import clip_tower_oracle as cto
+from oracle import clip_tower_train_oracle as ctt
+
+pytestmark = pytest.mark.gpu
+DEV = "cuda:0"
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HOOKS = os.path.join(ROOT, "tokenpacker_b200", "libtokenpacker_b200_clip_tower_train_hooks.so")
+GATE = 1.5e-2                                               # rel-RMS per gradient tensor: the projector's gate
+# q_proj / k_proj: their gradients go through the softmax, dS = P o (dP - D), a small difference of larger terms when the attention is
+# near uniform, as seeded N(0, 0.02) weights make it.  That amplifies the bf16 rounding of the FORWARD's q and k, which the oracle's
+# fp64 forward does not have: observed 1.4 - 2.0 % on q_proj and k_proj.weight, 0.2 - 1.2 % on everything else.  The attention
+# backward itself holds 0.3 - 0.6 % against fp64 computed from the same stored operands (test_attention_backward_against_fp64).
+GATE_QK = 2.5e-2
+
+
+def _gate(key):
+    return GATE_QK if "q_proj" in key or "k_proj" in key else GATE
+
+
+def _grad_error(got, ref, key):
+    """rel-RMS of one layer's gradient ``key``.  k_proj.bias has the exact gradient 0 (a constant added to every key moves all scores
+    of a row alike): its error is measured against v_proj.bias's gradient instead."""
+    if key == "self_attn.k_proj.bias":
+        return float((got[key].double() - ref[key]).norm() / ref["self_attn.v_proj.bias"].norm())
+    return _rel(got[key], ref[key])
+
+
+@pytest.fixture(scope="module")
+def hooks():
+    lib = C.CDLL(HOOKS)
+    p, i64 = C.c_void_p, C.c_int64
+    for name, args in {"tptt_attention_lse": [p, p, p, i64, p], "tptt_attention_bwd": [p, p, p, p, p, p, i64, p],
+                       "tptt_quick_gelu_bwd": [p, p, i64, p, p, p], "tptt_ln_bwd": [p, p, C.c_int, p, p, p, p, p, i64, p, p, p, p],
+                       "tptt_saved_offsets": [i64, C.POINTER(i64)]}.items():
+        getattr(lib, name).restype = C.c_int
+        getattr(lib, name).argtypes = args
+    return lib
+
+
+def _ptr(t):
+    return C.c_void_p(t.data_ptr())
+
+
+def _rel(got, ref):
+    ref = ref.double()
+    return float((got.double() - ref).norm() / ref.norm().clamp_min(1e-300))
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# attention backward
+# ------------------------------------------------------------------------------------------------------------------------------
+def _attention_fp64(qkv, dctx, n):
+    """fp64 forward and backward of the 577-token attention from the bf16 qkv (q pre-scaled) and dctx."""
+    x = qkv.double().view(n, 577, 3, 16, 64).permute(2, 0, 3, 1, 4)               # [3, n, 16, 577, 64]
+    q, k, v = x[0], x[1], x[2]
+    do = dctx.double().view(n, 577, 16, 64).transpose(1, 2)
+    s = q @ k.transpose(-1, -2)
+    p = torch.softmax(s, dim=-1)
+    o = p @ v
+    lse2 = torch.logsumexp(s, dim=-1) / torch.log(torch.tensor(2.0, dtype=torch.float64))
+    dv = p.transpose(-1, -2) @ do
+    dp = do @ v.transpose(-1, -2)
+    ds = p * (dp - (do * o).sum(-1, keepdim=True))
+    dq, dk = ds @ k, ds.transpose(-1, -2) @ q
+    back = lambda t: t.transpose(1, 2).reshape(n * 577, 1024)
+    return back(o), lse2, torch.cat([back(dq), back(dk), back(dv)], dim=1)
+
+
+def _attention_inputs(n):
+    g = torch.Generator(device=DEV).manual_seed(41)
+    qkv = torch.randn(n * 577 + 64, 3072, generator=g, device=DEV)
+    x = qkv[: n * 577].view(n, 577, 3, 16, 64)
+    x[:, :, 0] *= 0.35                                      # q carries the 1/8: scores of a few units
+    x[0, :, 0, 1] *= 4.0                                    # head 1 of crop 0: peaked softmax
+    x[0, :, 1, 3] *= 0.01                                   # head 3: one dominant key
+    x[0, 123, 1, 3] = 20.0
+    x[1, :, 0, 4] = 0.0                                     # head 4 of crop 1: all-equal logits.  The 63 zero-filled keys 577..639 score 0 as
+    x[1, :, 2, 4] = 1.0                                     # well: unmasked they would take 63/640 of every row's weight
+    if n > 2:
+        x[2, :, 2] *= 1e3                                   # crop 2's values are huge: crop 1's padded rows read zeros, never these
+    qkv[n * 577:] = 3e4                                     # rows after the last crop: never read
+    dctx = torch.randn(n * 577 + 64, 1024, generator=g, device=DEV)
+    dctx[n * 577:] = 3e4
+    return qkv.bfloat16(), dctx.bfloat16()
+
+
+def _run_attention(hooks, qkv, dctx, n):
+    ctx = torch.full((n * 577 + 8, 1024), float("nan"), device=DEV).bfloat16()
+    lse = torch.full((n, 16, 640), float("nan"), device=DEV)
+    delta = torch.full((n, 16, 640), float("nan"), device=DEV)
+    dqkv = torch.full((n * 577 + 8, 3072), float("nan"), device=DEV).bfloat16()
+    assert hooks.tptt_attention_lse(_ptr(qkv), _ptr(ctx), _ptr(lse), n, None) == 0
+    assert hooks.tptt_attention_bwd(_ptr(qkv), _ptr(lse), _ptr(ctx), _ptr(dctx), _ptr(delta), _ptr(dqkv), n, None) == 0
+    torch.cuda.synchronize()
+    return ctx, lse, dqkv
+
+
+def test_attention_backward_against_fp64(hooks):
+    n = 3
+    qkv, dctx = _attention_inputs(n)
+    ctx, lse, dqkv = _run_attention(hooks, qkv, dctx, n)
+    assert torch.isnan(dqkv[n * 577:].float()).all() and torch.isnan(lse[:, :, 577:]).all()      # nothing written past the crops / tokens
+    o_ref, lse_ref, d_ref = _attention_fp64(qkv[: n * 577], dctx[: n * 577], n)
+    assert float((lse[:, :, :577].double() - lse_ref).abs().max()) < 2e-2                        # log2 units; P is rounded to bf16 before its sum
+    got = dqkv[: n * 577].double()
+    assert torch.isfinite(got).all()
+    # P and dS are rounded to bf16 before the second products and the results once more: three 2^-9 roundings, summed over 577 terms
+    # of mixed sign; D comes from the bf16 ctx.  Where the softmax is one-hot (crop 0, heads 1 and 3) the true dS = P (dP - D) is a
+    # cancellation to almost nothing, so a head's error is bounded against the larger of its own RMS and a tenth of the RMS of its
+    # (crop, third) over all heads.
+    gb = got.view(n, 577, 3, 16, 64)
+    rb = d_ref.view(n, 577, 3, 16, 64)
+    err = (gb - rb).pow(2).mean(dim=(1, 4)).sqrt()                                               # [n, 3, 16]
+    scale = rb.pow(2).mean(dim=(1, 4)).sqrt()
+    block = rb.pow(2).mean(dim=(1, 3, 4)).sqrt()[:, :, None]                                     # [n, 3, 1]
+    ratio = err / torch.maximum(scale, 0.1 * block)
+    per_block = (gb - rb).pow(2).mean(dim=(1, 3, 4)).sqrt() / block[:, :, 0]
+    print(f"attention backward: rel-RMS per (crop, dq|dk|dv) {[[round(float(v), 5) for v in row] for row in per_block]}, worst head "
+          f"{float(ratio.max()):.2e} at {divmod(int(ratio.argmax()), 16)}, overall {_rel(got, d_ref):.2e}")
+    assert float(per_block.max()) < 1e-2, per_block
+    assert float(ratio.max()) < 3e-2, ratio
+    # the all-equal-logits head: P = 1/577 exactly on the real keys, so dV rows are colsum(dO) / 577; unmasked padding would give 1/640
+    dv4 = gb[1, :, 2, 4]
+    want = dctx[577: 2 * 577].double().view(577, 16, 64)[:, 4].sum(0) / 577
+    assert float((dv4 - want).abs().max()) <= 2.0 ** -7 * float(want.abs().max()) + 1e-6
+
+
+def test_attention_backward_crops_are_independent_and_deterministic(hooks):
+    n = 3
+    qkv, dctx = _attention_inputs(n)
+    _, lse, full = _run_attention(hooks, qkv, dctx, n)
+    _, lse2, again = _run_attention(hooks, qkv, dctx, n)
+    assert torch.equal(full[: n * 577], again[: n * 577]) and torch.equal(lse[:, :, :577], lse2[:, :, :577])
+    # crop 1 alone: its padded rows 577..639 are zero-filled in both calls, so the bits cannot depend on the neighbours
+    q1 = qkv[577: 2 * 577].clone()
+    d1 = dctx[577: 2 * 577].clone()
+    _, _, single = _run_attention(hooks, q1, d1, 1)
+    assert torch.equal(single[:577], full[577: 2 * 577])
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# elementwise backward kernels
+# ------------------------------------------------------------------------------------------------------------------------------
+def test_quick_gelu_backward_and_bias_gradient(hooks):
+    g = torch.Generator(device=DEV).manual_seed(43)
+    rows = 577 * 2 + 3
+    z = (torch.randn(rows, 4096, generator=g, device=DEV) * 3).bfloat16()
+    z[0, :8] = torch.tensor([-200.0, 200.0, -60.0, 60.0, -1e30, 1e30, 0.0, -0.75], device=DEV).bfloat16()
+    dh = torch.randn(rows, 4096, generator=g, device=DEV).bfloat16()
+    dz = dh.clone()
+    db = torch.empty(4096, device=DEV).bfloat16()
+    part = torch.empty(592 * 4096, device=DEV)
+    assert hooks.tptt_quick_gelu_bwd(_ptr(dz), _ptr(z), rows, _ptr(db), _ptr(part), None) == 0
+    torch.cuda.synchronize()
+    zd = z.double()
+    s = torch.sigmoid(1.702 * zd)
+    ref = dh.double() * s * (1 + 1.702 * zd * (1 - s))
+    assert torch.isfinite(dz.float()).all()
+    # __expf and the reciprocal: a few fp32 ulps; then one bf16 rounding
+    err = (dz.double() - ref).abs()
+    assert (err <= 2.0 ** -8 * ref.abs() + 1e-6 * dh.double().abs()).all(), float(err.max())
+    assert float(dz[0, 0]) == 0.0 and float(dz[0, 4]) == 0.0 and float(dz[0, 1]) == float(dh[0, 1]) and float(dz[0, 5]) == float(dh[0, 5])
+    col = dz.double().sum(0)                                # the sums are over the ROUNDED dz
+    assert float((db.double() - col).abs().max()) <= 2.0 ** -8 * float(col.abs().max()) + 1e-3
+
+
+@pytest.mark.parametrize("x_f32", [0, 1], ids=["layer_norm1", "layer_norm2"])
+def test_layernorm_backward_with_outlier_channels(hooks, x_f32):
+    g = torch.Generator(device=DEV).manual_seed(47 + x_f32)
+    rows = 577 * 3
+    x = torch.randn(rows, 1024, generator=g, device=DEV)
+    x[:, list(cto.OUTLIER_CHANNELS)] += torch.tensor([70.0, -60.0, 90.0, -50.0], device=DEV)
+    x = x if x_f32 else x.bfloat16()
+    gamma = (1 + 0.1 * torch.randn(1024, generator=g, device=DEV)).bfloat16()
+    gy = torch.randn(rows, 1024, generator=g, device=DEV).bfloat16()
+    add = torch.randn(rows, 1024, generator=g, device=DEV).bfloat16()
+    carry = torch.randn(rows, 1024, generator=g, device=DEV)
+    c32 = carry.clone()
+    c16 = torch.empty(rows, 1024, device=DEV).bfloat16()
+    part = torch.empty(296 * 3 * 1024, device=DEV)
+    dgam, dbet, dsum = (torch.empty(1024, device=DEV).bfloat16() for _ in range(3))
+    assert hooks.tptt_ln_bwd(_ptr(gy), _ptr(x), x_f32, _ptr(gamma), _ptr(add), _ptr(c32), _ptr(c16), _ptr(part), rows, _ptr(dgam), _ptr(dbet),
+                             _ptr(dsum), None) == 0
+    torch.cuda.synchronize()
+    xd = x.double().requires_grad_(True)
+    gd = gamma.double().requires_grad_(True)
+    bd = torch.zeros(1024, dtype=torch.float64, device=DEV, requires_grad=True)
+    y = torch.nn.functional.layer_norm(xd, (1024,), gd, bd, 1e-5)
+    y.backward(gy.double())
+    ref = carry.double() + add.double() + xd.grad
+    # fp32 arithmetic on 1024-wide rows whose statistics are dominated by four channels of +-50..90
+    assert _rel(c32, ref) < 1e-5
+    assert torch.equal(c16, c32.bfloat16())
+    for name, got, want in (("dgamma", dgam, gd.grad), ("dbeta", dbet, bd.grad), ("dsum", dsum, c16.double().sum(0))):
+        assert _rel(got, want) < 2.0 ** -8, name
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the tower
+# ------------------------------------------------------------------------------------------------------------------------------
+@pytest.fixture(scope="module")
+def weights():
+    return cto.round_bf16(cto.make_weights(23, seed=11, device=DEV))
+
+
+def _model(w, trainable_from=None):
+    model = cto.FakeCLIPVisionModel({k: v.bfloat16() for k, v in w.items()}).to(DEV)
+    if trainable_from is not None:
+        for name, p in model.named_parameters():
+            if "encoder.layers." in name and int(name.split("encoder.layers.")[1].split(".")[0]) >= trainable_from:
+                p.requires_grad_(True)
+    return model
+
+
+def _layer_grads(model, i):
+    named = dict(model.named_parameters())
+    keys = cto.layer_keys(i)
+    return {k: named["vision_model." + keys[k]].grad for k in ctt.PARAM_KEYS}
+
+
+def test_training_forward_has_the_inference_bits_and_saves_what_the_backward_reads(hooks, weights):
+    from tokenpacker_b200 import CLIPVisionTowerB200, _lib
+    lib = _lib.lib
+    n, k = 2, 2
+    model = _model(weights)
+    t = CLIPVisionTowerB200(model)
+    images = cto.make_images(n, seed=51, device=DEV).bfloat16()
+    with torch.no_grad():
+        ref = t.hidden_states(images)
+    packed, (w, _) = t._packed_weights(torch.device(DEV))
+    outs = [torch.empty_like(r) for r in ref]
+    saved_bytes, ws_bytes = lib.tp_clip_tower_train_saved_bytes(n, k), lib.tp_clip_tower_train_workspace_bytes(n, k)
+    saved = torch.full((saved_bytes,), 0xFF, dtype=torch.uint8, device=DEV)          # NaN poison
+    ws = torch.full((ws_bytes,), 0xFF, dtype=torch.uint8, device=DEV)
+    ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
+    _lib.check(lib.tp_clip_tower_forward_train(packed.data_ptr(), C.byref(w), images.data_ptr(), n, images.stride(0), k, ptrs, saved.data_ptr(),
+                                               saved_bytes, ws.data_ptr(), ws_bytes, None), "tp_clip_tower_forward_train")
+    torch.cuda.synchronize()
+    for a, b in zip(outs, ref):
+        assert torch.equal(a, b)
+    off = (C.c_int64 * 12)()
+    assert hooks.tptt_saved_offsets(n, off) == 0
+    M = n * 577
+    o = dict(zip(("pack", "x", "y1", "qkv", "lse", "ctx", "xp", "y2", "z", "h", "bytes", "w_qkv"), off))
+    assert saved_bytes == k * o["bytes"]
+    layer = 22                                                                        # the second saved set: input hidden_states[22]
+    base = o["bytes"]
+
+    def view(name, cols, dtype=torch.bfloat16):
+        size = torch.empty(0, dtype=dtype).element_size()
+        return saved[base + o[name]: base + o[name] + M * cols * size].view(dtype).view(M, cols)
+
+    p = ctt.layer_params(weights, layer, torch.float64, DEV)
+    x = view("x", 1024)
+    assert torch.equal(x.view(n, 577, 1024), ref[2])                                  # hidden_states[22], copied to the caller too
+    ln = lambda v, a, b: torch.nn.functional.layer_norm(v.double(), (1024,), p[a], p[b], 1e-5)
+    y1, qkv, ctx, xp, y2, z, h = (view(*a) for a in (("y1", 1024), ("qkv", 3072), ("ctx", 1024), ("xp", 1024, torch.float32), ("y2", 1024),
+                                                       ("z", 4096), ("h", 4096)))
+    w_qkv = torch.cat([p["self_attn.q_proj.weight"] / 8, p["self_attn.k_proj.weight"], p["self_attn.v_proj.weight"]])
+    b_qkv = torch.cat([p["self_attn.q_proj.bias"] / 8, p["self_attn.k_proj.bias"], p["self_attn.v_proj.bias"]])
+    packed_w = saved[base + o["pack"] + o["w_qkv"]: base + o["pack"] + o["w_qkv"] + 3072 * 1024 * 2].view(torch.bfloat16).view(3072, 1024)
+    assert torch.equal(packed_w.double(), w_qkv)                                      # rebuilt from the live parameters, q / 8 exact
+    o_ref, lse_ref, _ = _attention_fp64(qkv, torch.zeros(M, 1024, device=DEV), n)
+    lse = saved[base + o["lse"]: base + o["lse"] + n * 16 * 640 * 4].view(torch.float32).view(n, 16, 640)
+    zz = y2.double() @ p["mlp.fc1.weight"].T + p["mlp.fc1.bias"]
+    checks = {"y1": (y1, ln(x, "layer_norm1.weight", "layer_norm1.bias")), "qkv": (qkv, y1.double() @ w_qkv.T + b_qkv), "ctx": (ctx, o_ref),
+              "xp": (xp, x.double() + ctx.double() @ p["self_attn.out_proj.weight"].T + p["self_attn.out_proj.bias"]),
+              "y2": (y2, ln(xp, "layer_norm2.weight", "layer_norm2.bias")), "z": (z, zz), "h": (h, cto.quick_gelu(zz)),
+              "out": (outs[3].view(M, 1024), xp.double() + h.double() @ p["mlp.fc2.weight"].T + p["mlp.fc2.bias"])}
+    for name, (got, want) in checks.items():
+        assert torch.isfinite(got.float()).all(), name
+        # one bf16 rounding of an fp32-accumulated value (none for the fp32 x'); ctx adds the rounding of P
+        assert _rel(got, want) < (1e-5 if name == "xp" else 2.0 ** -6 if name == "ctx" else 2.0 ** -8), (name, _rel(got, want))
+    assert float((lse[:, :, :577].double() - lse_ref).abs().max()) < 2e-2
+    # h has the bits of the fused epilogue: quick_gelu of the UNROUNDED pre-activation, not of the stored z
+    assert torch.equal(outs[3], ref[3])
+
+
+@pytest.mark.parametrize("n", [1, 3])
+@pytest.mark.parametrize("k", [1, 4, 12, 23])
+def test_parameter_gradients_against_the_fp64_oracle(weights, n, k):
+    from tokenpacker_b200 import CLIPVisionTowerB200
+    first = 23 - k
+    model = _model(weights, trainable_from=first)
+    t = CLIPVisionTowerB200(model, trainable_layers=k)
+    images = cto.make_images(n, seed=60 + n, device=DEV).bfloat16()
+    with torch.no_grad():
+        ref_outs = CLIPVisionTowerB200(model).hidden_states(images)
+    g = torch.Generator(device=DEV).manual_seed(70 + k)
+    d_outs = {j: (torch.randn(n, 577, 1024, generator=g, device=DEV) * 0.1).bfloat16() for j in cto.OUT_LAYERS}
+    d_outs[16] = None                                                                 # an output the loss does not use
+    outs = t.hidden_states(images)
+    for a, b, j in zip(outs, ref_outs, cto.OUT_LAYERS):
+        assert torch.equal(a, b)
+        assert a.requires_grad == (j - 1 >= first), j                                 # detached at or below the first trainable layer's input
+    loss = sum((o.float() * d_outs[j].float()).sum() for o, j in zip(outs, cto.OUT_LAYERS) if d_outs[j] is not None and o.requires_grad)
+    loss.backward()
+    torch.cuda.synchronize()
+    ref, _ = ctt.parameter_gradients(weights, images.float(), k, d_outs, 23, torch.float64, DEV)
+    worst = {}
+    for i in range(first, 23):
+        got = _layer_grads(model, i)
+        for key in ctt.PARAM_KEYS:
+            assert got[key] is not None and torch.isfinite(got[key].float()).all(), (i, key)
+            r = _grad_error(got, ref[i - first], key)
+            worst[key] = max(worst.get(key, 0.0), r)
+    print(f"N={n} K={k}: worst rel-RMS per parameter kind: " + ", ".join(f"{a.split('.')[-2]}.{a.split('.')[-1]} {b:.2e}" for a, b in worst.items()))
+    assert all(r < _gate(key) for key, r in worst.items()), worst
+    for name, p in model.named_parameters():                                           # nothing below the first trainable layer gets a gradient
+        if "encoder.layers." not in name or int(name.split("encoder.layers.")[1].split(".")[0]) < first:
+            assert p.grad is None, name
+
+
+def test_frozen_parameters_none_gradients_and_determinism(weights):
+    from tokenpacker_b200 import CLIPVisionTowerB200
+    n, k = 2, 3
+    model = _model(weights, trainable_from=20)
+    named = dict(model.named_parameters())
+    frozen = ["vision_model." + cto.layer_keys(21)[key] for key in ("mlp.fc1.weight", "self_attn.q_proj.bias", "layer_norm2.weight")]
+    for name in frozen:
+        named[name].requires_grad_(False)
+    t = CLIPVisionTowerB200(model, trainable_layers=k)
+    images = cto.make_images(n, seed=81, device=DEV).bfloat16()
+
+    def step():
+        for p in model.parameters():
+            p.grad = None
+        outs = t.hidden_states(images)
+        outs[3].float().square().mean().backward()                                     # only hidden_states[23]: three None gradients upstream
+        torch.cuda.synchronize()
+        return {name: p.grad.clone() for name, p in model.named_parameters() if p.grad is not None}
+
+    a, b = step(), step()
+    assert set(a) == set(b) and all(torch.equal(a[name], b[name]) for name in a)       # bit determinism run to run
+    assert not set(frozen) & set(a)
+    assert len(a) == 3 * 16 - 3
+    # gradients accumulate like any autograd gradient: a second backward without clearing doubles them
+    outs = t.hidden_states(images)
+    outs[3].float().square().mean().backward()
+    name = "vision_model." + cto.layer_keys(22)["mlp.fc2.bias"]
+    assert torch.allclose(named[name].grad.float(), 2 * a[name].float(), rtol=2.0 ** -7, atol=0)
+    # under no_grad, and with nothing trainable requiring grad, the inference path runs
+    with torch.no_grad():
+        assert not t.hidden_states(images)[3].requires_grad
+    for p in model.parameters():
+        p.requires_grad_(False)
+    assert not t.hidden_states(images)[3].requires_grad
+    with pytest.raises(NotImplementedError, match="forward only"):
+        t.hidden_states(images.clone().requires_grad_(True))
+
+
+def test_default_tower_keeps_its_launches_and_memory(weights):
+    from tokenpacker_b200 import CLIPVisionTowerB200, _lib
+    model = _model(weights)
+    a, b = CLIPVisionTowerB200(model), CLIPVisionTowerB200(model, trainable_layers=4)
+    images = cto.make_images(2, seed=83, device=DEV).bfloat16()
+    with torch.no_grad():
+        a.hidden_states(images), b.hidden_states(images)                               # caches built
+        stats = []
+        for t in (a, b):
+            torch.cuda.synchronize()
+            torch.cuda.reset_peak_memory_stats()
+            c0 = _lib.lib.tp_launch_count()
+            out = t.hidden_states(images)
+            torch.cuda.synchronize()
+            stats.append((_lib.lib.tp_launch_count() - c0, torch.cuda.max_memory_allocated(), out))
+            del out
+    assert stats[0][0] == stats[1][0] and all(torch.equal(x, y) for x, y in zip(stats[0][2], stats[1][2]))
+    assert abs(stats[0][1] - stats[1][1]) <= 4 * 2 * 577 * 1024 * 2                     # the previous call's outputs may still be alive
+
+
+def test_uint8_images_through_tower_and_projector_backward(weights):
+    """Decoded images -> hd_preprocess_batch -> tower (last 2 layers trainable) -> packed projector output with input_grad -> loss ->
+    backward.  The projector hands the tower the gradients of the four hidden states; the tower's parameter gradients are compared
+    with the fp64 oracle driven by those same four gradients, and the projector's own gradients with a run fed detached hidden states."""
+    from tokenpacker_b200 import CLIPVisionTowerB200, TokenPackerB200, hd_preprocess_batch
+    g = torch.Generator(device=DEV).manual_seed(91)
+    images = [torch.randint(0, 256, (h_, w_, 3), generator=g, device=DEV, dtype=torch.uint8) for h_, w_ in ((336, 336), (400, 600))]
+    torch.manual_seed(7)
+    proj = TokenPackerB200(hidden_size=1024, scale_factor=2).to(DEV, torch.bfloat16).train()
+    proj.input_grad = True
+    sep, ret = torch.randn(1024, device=DEV).bfloat16(), torch.randn(1024, device=DEV).bfloat16()
+    model = _model(weights, trainable_from=21)
+    t = CLIPVisionTowerB200(model, trainable_layers=2)
+    with torch.no_grad():
+        crops, hb, wb = hd_preprocess_batch(images, patch_num=9, dtype=torch.bfloat16)
+    hs = t.hidden_states(crops)
+    for h in hs:
+        if h.requires_grad:
+            h.retain_grad()
+    out = proj.forward_hidden_states_packed(list(hs), hb, wb, sep, ret)[0]
+    out.float().square().mean().backward()
+    torch.cuda.synchronize()
+    assert hs[0].grad is None and hs[1].grad is None and hs[2].grad is not None and hs[3].grad is not None
+    d_outs = {12: None, 16: None, 22: hs[2].grad, 23: hs[3].grad}
+    ref, _ = ctt.parameter_gradients(weights, crops.float(), 2, d_outs, 23, torch.float64, DEV)
+    for i in (21, 22):
+        got = _layer_grads(model, i)
+        for key in ctt.PARAM_KEYS:
+            assert _grad_error(got, ref[i - 21], key) < _gate(key), (i, key, _grad_error(got, ref[i - 21], key))
+    proj_grads = {name: p.grad.clone() for name, p in proj.named_parameters() if p.grad is not None}
+    assert proj_grads
+    for p in proj.parameters():
+        p.grad = None
+    proj.forward_hidden_states_packed([h.detach() for h in hs], hb, wb, sep, ret)[0].float().square().mean().backward()
+    for name, p in proj.named_parameters():
+        if p.grad is not None:
+            assert torch.equal(p.grad, proj_grads[name]), name

@@ -2,8 +2,8 @@
 
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
 Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
-include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h, include/tokenpacker_b200_clip_tower.h and
-include/tokenpacker_b200_clip_tower_f16.h one to one.
+include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h, include/tokenpacker_b200_clip_tower.h,
+include/tokenpacker_b200_clip_tower_f16.h and include/tokenpacker_b200_clip_tower_train.h one to one.
 """
 from __future__ import annotations
 
@@ -190,6 +190,22 @@ CLIP_TOWER_F16_SIGNATURES = {
                                             C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
+# the same for include/tokenpacker_b200_clip_tower_train.h (training the last K layers of the tower)
+class TpClipTowerLayerGrads(C.Structure):
+    """tp_clip_tower_layer_grads: one gradient destination per parameter of a layer (None: not wanted)."""
+    _fields_ = [(name, C.c_void_p) for name, _ in CLIP_TOWER_LAYER_FIELDS]
+
+
+CLIP_TOWER_TRAIN_SIGNATURES = {
+    "tp_clip_tower_train_saved_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "tp_clip_tower_train_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "tp_clip_tower_backward_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int]),
+    "tp_clip_tower_forward_train": (C.c_int, [C.c_void_p, C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_int64, C.c_int64, C.c_int,
+                                              C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "tp_clip_tower_backward": (C.c_int, [C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_int64, C.c_int, C.POINTER(C.c_void_p),
+                                         C.POINTER(TpClipTowerLayerGrads), C.c_void_p, C.c_size_t, C.c_void_p]),
+}
+
 
 def _load():
     if not os.path.exists(LIB_PATH):
@@ -198,7 +214,8 @@ def _load():
             "(or `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
-                                      **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES}.items():
+                                      **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES,
+                                      **CLIP_TOWER_TRAIN_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

@@ -14,6 +14,7 @@
 #include "../../include/tokenpacker_b200.h"
 #include "../../include/tokenpacker_b200_clip_tower.h"
 #include "../../include/tokenpacker_b200_clip_tower_f16.h"
+#include "../../include/tokenpacker_b200_clip_tower_train.h"
 #include "../../include/tokenpacker_b200_clip_u8.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"
@@ -22,6 +23,7 @@
 #include "tp_kernels.cuh"
 #include "tp_backward.cuh"
 #include "tp_clip_tower.cuh"
+#include "tp_clip_tower_train.cuh"
 
 namespace {
 
@@ -1902,3 +1904,4 @@ int tp_hd_fill_separators(void* out, int hidden, const int64_t* sep_rows, int64_
 }  // extern "C"
 
 #include "tp_clip_tower.inl"
+#include "tp_clip_tower_train.inl"

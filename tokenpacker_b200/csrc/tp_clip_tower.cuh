@@ -20,6 +20,7 @@ constexpr int kClipPatchLd = 592;           // patch rows padded to a 16-byte mu
 constexpr int kClipHeads = 16;
 constexpr int kClipHeadDim = 64;
 constexpr float kClipLnEps = 1e-5f;
+constexpr int kClipStatLd = 640;            // tokens per (crop, head) row of the training path's softmax statistics: 5 query blocks of 128
 
 // One thread per (patch row, channel, kernel row): 14 consecutive pixels in, 14 consecutive patch-row elements out.  bf16 crops into
 // f16 patch rows are converted as images.to(torch.float16) does (clip_encoder.py:59): through fp32, one round-to-nearest-even.
@@ -155,6 +156,8 @@ __global__ void clip_layernorm_kernel(const T* __restrict__ x, long long rows, c
 //   S = Q K^T (wgmma m64n128k16, both K-major), keys >= 577 set to -inf BEFORE the row max (a zero-filled key scores 0 and would take
 //   weight), online softmax in fp32 (exp2 on log2(e)-scaled scores), P rounded to bf16 into shared memory (K-major, 128-byte
 //   swizzle), O += P V (wgmma m64n64k16, V as the MN-major B operand).  The row sum is taken over the ROUNDED P that multiplies V.
+// kLse (the training forward): also writes lse[crop][head][t] = m log2(e) + log2(l), the log2 of the softmax denominator on the scale of
+// the exp2 above ([N, 16, 640] fp32, tokens >= 577 not written), from which the backward recomputes P = exp2(s log2(e) - lse).
 // ------------------------------------------------------------------------------------------------
 constexpr int kAttnKeyBoxes = 10;                         // 640 >= 577 keys in boxes of 64
 constexpr int kAttnBoxBytes = 64 * 128;                   // 64 tokens x 64 channels bf16
@@ -168,9 +171,9 @@ struct ClipAttnSmem {
 };
 static_assert(ClipAttnSmem::kBytes <= 232448, "shared memory budget of an sm_90 SM (227 KiB)");
 
-template <typename T>
+template <typename T, bool kLse = false>
 __global__ void __launch_bounds__(256, 1)
-clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, T* __restrict__ ctx) {
+clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, T* __restrict__ ctx, float* __restrict__ lse) {
   constexpr bool kF16 = std::is_same_v<T, __half>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -277,6 +280,7 @@ clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, T* __restrict__ c
   for (int h = 0; h < 2; ++h) {
     const int t = qb * 128 + wg * 64 + 16 * warp + g + 8 * h;
     if (t >= kClipTokens) continue;
+    if (kLse && q == 0) lse[(static_cast<long long>(crop) * kClipHeads + head) * kClipStatLd + t] = fmaf(m[h], kLog2e, lg2_approx(l[h]));
     T* dst = ctx + (static_cast<long long>(crop) * kClipTokens + t) * 1024 + head * kClipHeadDim + 2 * q;
 #pragma unroll
     for (int i = 2 * h; i < 32; i += 4)

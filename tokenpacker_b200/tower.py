@@ -12,6 +12,14 @@ and a ``.config`` carrying its fields is accepted.
 ``CLIPVisionTowerB200(model, dtype=torch.float16)`` runs the tower in fp16, as the reference's evaluation and serving scripts do
 (``vision_tower.to(dtype=torch.float16)``, llava/eval/model_vqa_loader.py): the hidden states come back fp16, and the caller casts them
 to bf16 for the projector as clip_encoder.py does (``[h.to(torch.bfloat16) for h in hs]``).
+
+``CLIPVisionTowerB200(model, trainable_layers=K)`` trains the last K encoder layers (include/tokenpacker_b200_clip_tower_train.h):
+under ``torch.enable_grad()`` the four hidden states are attached to autograd, and their backward writes the gradients of the
+parameters of layers 23 - K .. 22 that require grad.  With the projector's ``input_grad`` this closes the loop:
+
+    tower = CLIPVisionTowerB200(vision_tower, trainable_layers=4)
+    proj.input_grad = True
+    proj.forward_hidden_states(tower.hidden_states(crops)).float().square().mean().backward()
 """
 from __future__ import annotations
 
@@ -27,6 +35,49 @@ from ._lib import check, lib
 _TOKENS = 577
 _IMAGE = 336
 _OUT_LAYERS = (12, 16, 22, 23)
+
+
+class _TowerTrainFunction(torch.autograd.Function):
+    """hidden_states 12 / 16 / 22 / 23 with the last K layers under autograd.  Inputs after the first four are the 16 K parameters of
+    the trainable layers, in _lib.CLIP_TOWER_LAYER_FIELDS order, layer 23 - K first."""
+
+    @staticmethod
+    def forward(ctx, tower, x, packed, w, *params):
+        k, n, device = tower.trainable_layers, x.shape[0], x.device
+        outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=torch.bfloat16, device=device) for _ in _OUT_LAYERS)
+        saved_bytes = lib.tp_clip_tower_train_saved_bytes(n, k)
+        ws_bytes = lib.tp_clip_tower_train_workspace_bytes(n, k)
+        saved = torch.empty(saved_bytes, dtype=torch.uint8, device=device)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            check(lib.tp_clip_tower_forward_train(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), k, ptrs, saved.data_ptr(),
+                                                  saved_bytes, ws.data_ptr(), ws_bytes, stream), "tp_clip_tower_forward_train")
+        ctx.w, ctx.saved, ctx.k, ctx.n, ctx.params = w, saved, k, n, params
+        ctx.set_materialize_grads(False)                # an output nobody used arrives as None, not as a tensor of zeros
+        # hidden_states[j] is the output of layer j - 1: below the first trainable layer (23 - k) nothing of it depends on a trainable parameter
+        frozen = [o for o, j in zip(outs, _OUT_LAYERS) if j - 1 < _lib.CLIP_TOWER_LAYERS - k]
+        ctx.mark_non_differentiable(*frozen)
+        return outs
+
+    @staticmethod
+    def backward(ctx, *d_outs):
+        k, n, device = ctx.k, ctx.n, ctx.saved.device
+        d_outs = [None if g is None else g.to(torch.bfloat16).contiguous() for g in d_outs]
+        d_ptrs = (C.c_void_p * 4)(*[None if g is None else g.data_ptr() for g in d_outs])
+        per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
+        grads = [torch.empty_like(p) if ctx.needs_input_grad[4 + i] else None for i, p in enumerate(ctx.params)]
+        g_structs = (_lib.TpClipTowerLayerGrads * k)()
+        for t in range(k):
+            g_structs[t] = _lib.TpClipTowerLayerGrads(*[None if g is None else g.data_ptr() for g in grads[t * per:(t + 1) * per]])
+        ws_bytes = lib.tp_clip_tower_backward_workspace_bytes(n, k)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            check(lib.tp_clip_tower_backward(C.byref(ctx.w), ctx.saved.data_ptr(), n, k, d_ptrs, g_structs, ws.data_ptr(), ws_bytes, stream),
+                  "tp_clip_tower_backward")
+        return (None, None, None, None) + tuple(grads)
 
 
 def _check_config(cfg):
@@ -54,12 +105,21 @@ class CLIPVisionTowerB200(nn.Module):
     The wrapped model stays the owner of the parameters (``self.vision_model``).  A derived cache (about 147 MB: per layer the q/k/v
     concatenation — with q scaled by 1/8 in bf16 —, and the biases in fp32) is keyed on the compute precision and every parameter's
     ``(data_ptr, _version, dtype)``, and dropped by ``load_state_dict``, ``.to()`` / ``.cuda()`` / ``.half()`` and
-    ``invalidate_packed()``."""
+    ``invalidate_packed()``.
 
-    def __init__(self, vision_model: nn.Module, dtype: torch.dtype | None = None):
+    trainable_layers: K in 0 .. 23, bf16 only.  0 (the default): forward only.  K > 0: encoder layers 23 - K .. 22 are trainable: see
+    ``hidden_states``.  Layers 0 .. 22 - K, the embeddings and pre_layrnorm stay frozen whatever their ``requires_grad`` says: they
+    get no gradient."""
+
+    def __init__(self, vision_model: nn.Module, dtype: torch.dtype | None = None, trainable_layers: int = 0):
         super().__init__()
         if dtype not in (None, torch.bfloat16, torch.float16):
             raise ValueError(f"CLIPVisionTowerB200 computes in torch.bfloat16 (dtype=None) or torch.float16, not {dtype!r}")
+        if not isinstance(trainable_layers, int) or isinstance(trainable_layers, bool) or not 0 <= trainable_layers <= _lib.CLIP_TOWER_LAYERS:
+            raise ValueError(f"trainable_layers = {trainable_layers!r}: expected an int in 0 .. {_lib.CLIP_TOWER_LAYERS}")
+        if trainable_layers > 0 and dtype == torch.float16:
+            raise ValueError("trainable_layers > 0 needs the bf16 tower: no released recipe trains CLIP in fp16 (its gradients underflow "
+                             "without loss scaling), so the fp16 tower is forward only")
         _check_config(getattr(vision_model, "config", None))
         named = dict(vision_model.named_parameters())
         prefix = "vision_model." if "vision_model.embeddings.class_embedding" in named else ""
@@ -71,6 +131,7 @@ class CLIPVisionTowerB200(nn.Module):
             raise NotImplementedError(f"not a CLIPVisionModel: parameters {missing[:3]} are missing")
         self.vision_model = vision_model
         self.dtype = torch.float16 if dtype == torch.float16 else torch.bfloat16
+        self.trainable_layers = trainable_layers
         self._names = names
         self._packed = None
         self._packed_key = None
@@ -92,6 +153,25 @@ class CLIPVisionTowerB200(nn.Module):
     def _params(self):
         named = dict(self.vision_model.named_parameters())
         return [named[n] for n in self._names]
+
+    def _trainable_params(self):
+        """The 16 K parameters of layers 23 - K .. 22, layer by layer in _lib.CLIP_TOWER_LAYER_FIELDS order."""
+        per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
+        first = len(_lib.CLIP_TOWER_FIELDS) + (_lib.CLIP_TOWER_LAYERS - self.trainable_layers) * per
+        return self._params()[first:] if self.trainable_layers > 0 else []
+
+    def _live_weights(self, w, train_params, device):
+        """A copy of the weight struct whose trainable layers point at the live parameters."""
+        for p in train_params:
+            if p.dtype != torch.bfloat16 or p.device != device or not p.is_contiguous() or p.data_ptr() % 16 != 0:
+                raise ValueError("the trainable layers' parameters are read in place: they must be contiguous, 16-byte aligned bf16 tensors "
+                                 "on the crops' device")
+        live = _lib.TpClipTowerWeights.from_buffer_copy(w)
+        per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
+        first = _lib.CLIP_TOWER_LAYERS - self.trainable_layers
+        for t in range(self.trainable_layers):
+            live.layers[first + t] = _lib.TpClipTowerLayer(*[p.data_ptr() for p in train_params[t * per:(t + 1) * per]])
+        return live
 
     def _packed_weights(self, device):
         params = self._params()
@@ -127,11 +207,18 @@ class CLIPVisionTowerB200(nn.Module):
         """images: [N, 3, 336, 336] CUDA crops (bf16 read in place, any crop stride; other dtypes cast to bf16).  Returns the tuple
         (hidden_states[12], [16], [22], [23]), each bf16 [N, 577, 1024] with the CLS row.
         With dtype=torch.float16: bf16 and fp16 crops are read in place (bf16 ones converted as ``images.to(torch.float16)`` rounds
-        them), other dtypes cast to fp16, and the four hidden states are fp16."""
+        them), other dtypes cast to fp16, and the four hidden states are fp16.
+        With trainable_layers = K > 0, under ``torch.enable_grad()`` and when a parameter of layers 23 - K .. 22 requires grad: the same
+        four tensors with the same bits, attached to autograd (those at or below the first trainable layer's input detached); their
+        backward takes up to four gradients (None allowed) and gives every such parameter that requires grad its gradient.  The trainable
+        layers' parameters must be bf16 CUDA tensors, contiguous and 16-byte aligned: they are read in place, and what is derived from
+        them is rebuilt by every call.  The crops get no gradient."""
         if not isinstance(images, torch.Tensor) or images.dim() != 4 or tuple(images.shape[1:]) != (3, _IMAGE, _IMAGE):
             shape = tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__
             raise ValueError(f"expected crops [N,3,336,336], got {shape}")
-        if torch.is_grad_enabled() and (images.requires_grad or any(p.requires_grad for p in self._params())):
+        train_params = self._trainable_params() if torch.is_grad_enabled() else []
+        train = any(p.requires_grad for p in train_params)
+        if torch.is_grad_enabled() and (images.requires_grad or (self.trainable_layers == 0 and any(p.requires_grad for p in self._params()))):
             raise NotImplementedError("CLIPVisionTowerB200 is forward only (the tower is frozen in every TokenPacker recipe): run it under "
                                       "torch.no_grad(), or detach the crops and freeze the tower's parameters")
         if not images.is_cuda:
@@ -147,6 +234,8 @@ class CLIPVisionTowerB200(nn.Module):
             if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
                 x = x.contiguous()
             packed, (w, _) = self._packed_weights(device)
+            if train:
+                return _TowerTrainFunction.apply(self, x, packed, self._live_weights(w, train_params, device), *train_params)
             ws_bytes = lib.tp_clip_tower_workspace_bytes(n)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
             ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
