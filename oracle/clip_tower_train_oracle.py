@@ -69,3 +69,14 @@ def parameter_gradients(w, images, k, d_outs, n_layers=23, dtype=torch.float64, 
     full = {j: below[j] for j in cto.OUT_LAYERS if j <= first}
     full.update({j: h.detach() for j, h in hs.items()})
     return [{key: p[key].grad for key in PARAM_KEYS} for p in params], full
+
+
+def parameter_gradients_chunked(w, images, k, d_outs, chunk, n_layers=23, dtype=torch.float64, device="cpu"):
+    """parameter_gradients over ``chunk`` crops at a time, summed: the loss is a sum over crops, so this is the same gradient with
+    the attention probabilities of ``chunk`` crops alive at once instead of all of them (fp64 P is 21 MB per crop and head)."""
+    total = None
+    for c0 in range(0, images.shape[0], chunk):
+        part = {j: None if d is None else d[c0:c0 + chunk] for j, d in d_outs.items()}
+        grads, _ = parameter_gradients(w, images[c0:c0 + chunk], k, part, n_layers, dtype, device)
+        total = grads if total is None else [{key: a[key] + b[key] for key in PARAM_KEYS} for a, b in zip(total, grads)]
+    return total

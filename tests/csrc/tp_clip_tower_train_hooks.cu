@@ -52,4 +52,32 @@ TP_API int tptt_saved_offsets(int64_t n, int64_t* out) {
   return TP_OK;
 }
 
+// Byte offsets inside a tp_clip_tower_backward workspace over n crops: carry32, carry16, dh, g, delta, ln_part, col_part, splitk,
+// unused_grad; out[9] = its total size
+TP_API int tptt_bwd_offsets(int64_t n, int64_t* out) {
+  if (n <= 0 || out == nullptr) return TP_ERR_INVALID_ARGUMENT;
+  const ClipBwdLayout B = clip_bwd_layout(n);
+  const size_t o[10] = {B.carry32, B.carry16, B.dh, B.g, B.delta, B.ln_part, B.col_part, B.splitk, B.unused_grad, B.total};
+  for (int i = 0; i < 10; ++i) out[i] = static_cast<int64_t>(o[i]);
+  return TP_OK;
+}
+
+// The backward of encoder layer `layer` alone (run_clip_layer_backward, as tp_clip_tower_backward runs it), from its saved set
+// `saved_set` of a tp_clip_tower_forward_train call over n crops, up to step last_step (1 .. 8, the numbering of
+// tp_clip_tower_train.inl).  The carry is NOT initialised: the caller writes carry32 and carry16 = bf16(carry32) into ws, so a test can
+// start from fp32 values bf16 cannot represent.  d_x: the caller's gradient of the layer's input hidden state (or NULL).
+TP_API int tptt_layer_backward(const tp_clip_tower_weights* w, int layer, const void* saved_set, int64_t n, const void* d_x,
+                               const tp_clip_tower_layer_grads* grads, void* ws, size_t ws_bytes, int last_step, void* stream) {
+  if (w == nullptr || saved_set == nullptr || grads == nullptr || ws == nullptr || n <= 0 || layer < 0 || layer >= TP_CLIP_TOWER_LAYERS ||
+      last_step < 1 || last_step > 8 || !clip_weights_complete(w))
+    return TP_ERR_INVALID_ARGUMENT;
+  if ((reinterpret_cast<uintptr_t>(saved_set) & 255) != 0 || (reinterpret_cast<uintptr_t>(ws) & 255) != 0) return TP_ERR_INVALID_ARGUMENT;
+  const ClipBwdLayout B = clip_bwd_layout(n);
+  if (ws_bytes < B.total) return TP_ERR_WORKSPACE_TOO_SMALL;
+  DeviceInfo dev;
+  TP_TRY(device_info(&dev));
+  return run_clip_layer_backward(w->layers[layer], static_cast<const uint8_t*>(saved_set), clip_saved_layout(n), d_x, *grads,
+                                 static_cast<uint8_t*>(ws), B, n, dev.sms, static_cast<cudaStream_t>(stream), last_step);
+}
+
 }  // extern "C"

@@ -289,6 +289,16 @@ def test_training_forward_has_the_inference_bits_and_saves_what_the_backward_rea
 @pytest.mark.parametrize("n", [1, 3])
 @pytest.mark.parametrize("k", [1, 4, 12, 23])
 def test_parameter_gradients_against_the_fp64_oracle(weights, n, k):
+    _parameter_gradients_case(weights, n, k)
+
+
+def test_parameter_gradients_at_a_split_k_batch(weights):
+    """29 crops (577 N = 16733 >= 16384 rows): the 1024 x 1024 weight gradients of both layers run split-K, as at every batch the
+    benchmark and HD training use; the same gates against the oracle, evaluated four crops at a time."""
+    _parameter_gradients_case(weights, 29, 2)
+
+
+def _parameter_gradients_case(weights, n, k):
     from tokenpacker_b200 import CLIPVisionTowerB200
     first = 23 - k
     model = _model(weights, trainable_from=first)
@@ -306,7 +316,7 @@ def test_parameter_gradients_against_the_fp64_oracle(weights, n, k):
     loss = sum((o.float() * d_outs[j].float()).sum() for o, j in zip(outs, cto.OUT_LAYERS) if d_outs[j] is not None and o.requires_grad)
     loss.backward()
     torch.cuda.synchronize()
-    ref, _ = ctt.parameter_gradients(weights, images.float(), k, d_outs, 23, torch.float64, DEV)
+    ref = ctt.parameter_gradients_chunked(weights, images.float(), k, d_outs, 4, 23, torch.float64, DEV)
     worst = {}
     for i in range(first, 23):
         got = _layer_grads(model, i)
