@@ -15,6 +15,7 @@
 #include "../../include/tokenpacker_b200_clip_tower.h"
 #include "../../include/tokenpacker_b200_clip_tower_f16.h"
 #include "../../include/tokenpacker_b200_clip_tower_train.h"
+#include "../../include/tokenpacker_b200_clip_tower_ckpt.h"
 #include "../../include/tokenpacker_b200_clip_u8.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"
@@ -1905,3 +1906,4 @@ int tp_hd_fill_separators(void* out, int hidden, const int64_t* sep_rows, int64_
 
 #include "tp_clip_tower.inl"
 #include "tp_clip_tower_train.inl"
+#include "tp_clip_tower_ckpt.inl"

@@ -20,6 +20,10 @@ parameters of layers 23 - K .. 22 that require grad.  With the projector's ``inp
     tower = CLIPVisionTowerB200(vision_tower, trainable_layers=4)
     proj.input_grad = True
     proj.forward_hidden_states(tower.hidden_states(crops)).float().square().mean().backward()
+
+When the wrapped model asks for gradient checkpointing (``vision_tower.gradient_checkpointing_enable()``, as the reference's recipes
+do with ``--gradient_checkpointing True``), that training step keeps only each trainable layer's input and derived weights and
+recomputes the rest in the backward (include/tokenpacker_b200_clip_tower_ckpt.h): less memory, more time, the same bits.
 """
 from __future__ import annotations
 
@@ -37,24 +41,32 @@ _IMAGE = 336
 _OUT_LAYERS = (12, 16, 22, 23)
 
 
+_NUM_FN_INPUTS = 5                                      # _TowerTrainFunction's inputs before the parameters
+
+
 class _TowerTrainFunction(torch.autograd.Function):
-    """hidden_states 12 / 16 / 22 / 23 with the last K layers under autograd.  Inputs after the first four are the 16 K parameters of
-    the trainable layers, in _lib.CLIP_TOWER_LAYER_FIELDS order, layer 23 - K first."""
+    """hidden_states 12 / 16 / 22 / 23 with the last K layers under autograd.  Inputs after the first five are the 16 K parameters of
+    the trainable layers, in _lib.CLIP_TOWER_LAYER_FIELDS order, layer 23 - K first.  checkpoint: keep only each trainable layer's
+    checkpoint (include/tokenpacker_b200_clip_tower_ckpt.h) instead of its full saved set; the backward follows the forward's mode."""
 
     @staticmethod
-    def forward(ctx, tower, x, packed, w, *params):
+    def forward(ctx, tower, x, packed, w, checkpoint, *params):
         k, n, device = tower.trainable_layers, x.shape[0], x.device
         outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=torch.bfloat16, device=device) for _ in _OUT_LAYERS)
-        saved_bytes = lib.tp_clip_tower_train_saved_bytes(n, k)
-        ws_bytes = lib.tp_clip_tower_train_workspace_bytes(n, k)
+        if checkpoint:
+            forward, name = lib.tp_clip_tower_forward_ckpt, "tp_clip_tower_forward_ckpt"
+            saved_bytes, ws_bytes = lib.tp_clip_tower_ckpt_saved_bytes(n, k), lib.tp_clip_tower_workspace_bytes(n)
+        else:
+            forward, name = lib.tp_clip_tower_forward_train, "tp_clip_tower_forward_train"
+            saved_bytes, ws_bytes = lib.tp_clip_tower_train_saved_bytes(n, k), lib.tp_clip_tower_train_workspace_bytes(n, k)
         saved = torch.empty(saved_bytes, dtype=torch.uint8, device=device)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
         ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            check(lib.tp_clip_tower_forward_train(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), k, ptrs, saved.data_ptr(),
-                                                  saved_bytes, ws.data_ptr(), ws_bytes, stream), "tp_clip_tower_forward_train")
-        ctx.w, ctx.saved, ctx.k, ctx.n, ctx.params = w, saved, k, n, params
+            check(forward(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), k, ptrs, saved.data_ptr(), saved_bytes, ws.data_ptr(),
+                          ws_bytes, stream), name)
+        ctx.w, ctx.saved, ctx.k, ctx.n, ctx.params, ctx.checkpoint = w, saved, k, n, params, checkpoint
         ctx.set_materialize_grads(False)                # an output nobody used arrives as None, not as a tensor of zeros
         # hidden_states[j] is the output of layer j - 1: below the first trainable layer (23 - k) nothing of it depends on a trainable parameter
         frozen = [o for o, j in zip(outs, _OUT_LAYERS) if j - 1 < _lib.CLIP_TOWER_LAYERS - k]
@@ -67,17 +79,27 @@ class _TowerTrainFunction(torch.autograd.Function):
         d_outs = [None if g is None else g.to(torch.bfloat16).contiguous() for g in d_outs]
         d_ptrs = (C.c_void_p * 4)(*[None if g is None else g.data_ptr() for g in d_outs])
         per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
-        grads = [torch.empty_like(p) if ctx.needs_input_grad[4 + i] else None for i, p in enumerate(ctx.params)]
+        grads = [torch.empty_like(p) if ctx.needs_input_grad[_NUM_FN_INPUTS + i] else None for i, p in enumerate(ctx.params)]
         g_structs = (_lib.TpClipTowerLayerGrads * k)()
         for t in range(k):
             g_structs[t] = _lib.TpClipTowerLayerGrads(*[None if g is None else g.data_ptr() for g in grads[t * per:(t + 1) * per]])
-        ws_bytes = lib.tp_clip_tower_backward_workspace_bytes(n, k)
+        if ctx.checkpoint:
+            backward, name, ws_bytes = lib.tp_clip_tower_backward_ckpt, "tp_clip_tower_backward_ckpt", lib.tp_clip_tower_ckpt_backward_workspace_bytes(n, k)
+        else:
+            backward, name, ws_bytes = lib.tp_clip_tower_backward, "tp_clip_tower_backward", lib.tp_clip_tower_backward_workspace_bytes(n, k)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            check(lib.tp_clip_tower_backward(C.byref(ctx.w), ctx.saved.data_ptr(), n, k, d_ptrs, g_structs, ws.data_ptr(), ws_bytes, stream),
-                  "tp_clip_tower_backward")
-        return (None, None, None, None) + tuple(grads)
+            check(backward(C.byref(ctx.w), ctx.saved.data_ptr(), n, k, d_ptrs, g_structs, ws.data_ptr(), ws_bytes, stream), name)
+        return (None,) * _NUM_FN_INPUTS + tuple(grads)
+
+
+def wants_gradient_checkpointing(vision_model: nn.Module) -> bool:
+    """Whether the wrapped model asks for gradient checkpointing: some submodule has ``gradient_checkpointing`` truthy and is in
+    training mode.  That is the condition under which transformers' own CLIPEncoder recomputes its layers
+    (``CLIPVisionModel.gradient_checkpointing_enable()`` sets ``encoder.gradient_checkpointing``), and
+    ``PreTrainedModel.is_gradient_checkpointing`` is the same test over ``modules()``."""
+    return any(bool(getattr(m, "gradient_checkpointing", False)) and m.training for m in vision_model.modules())
 
 
 def _check_config(cfg):
@@ -109,7 +131,12 @@ class CLIPVisionTowerB200(nn.Module):
 
     trainable_layers: K in 0 .. 23, bf16 only.  0 (the default): forward only.  K > 0: encoder layers 23 - K .. 22 are trainable: see
     ``hidden_states``.  Layers 0 .. 22 - K, the embeddings and pre_layrnorm stay frozen whatever their ``requires_grad`` says: they
-    get no gradient."""
+    get no gradient.
+
+    Gradient checkpointing has no switch of its own: the tower follows the wrapped model's (``gradient_checkpointing_enable()`` /
+    ``_disable()``, see ``wants_gradient_checkpointing``).  Checkpointing trades time for memory and no property of the input decides
+    between them, so the choice stays with the switch the model and the recipe that sets it already own; a second option here could
+    only disagree with it."""
 
     def __init__(self, vision_model: nn.Module, dtype: torch.dtype | None = None, trainable_layers: int = 0):
         super().__init__()
@@ -212,7 +239,11 @@ class CLIPVisionTowerB200(nn.Module):
         four tensors with the same bits, attached to autograd (those at or below the first trainable layer's input detached); their
         backward takes up to four gradients (None allowed) and gives every such parameter that requires grad its gradient.  The trainable
         layers' parameters must be bf16 CUDA tensors, contiguous and 16-byte aligned: they are read in place, and what is derived from
-        them is rebuilt by every call.  The crops get no gradient."""
+        them is rebuilt by every call.  The crops get no gradient.
+        When, in addition, the wrapped model asks for gradient checkpointing (``wants_gradient_checkpointing``, read at every call),
+        the step keeps per trainable layer only its input and its derived weights (1.2 MB per crop plus 6.3 MB, against 20.1 MB per
+        crop), and the backward recomputes each layer's intermediates before its gradients: the outputs and every gradient have the same
+        bits as without it.  A graph keeps the mode it was built with."""
         if not isinstance(images, torch.Tensor) or images.dim() != 4 or tuple(images.shape[1:]) != (3, _IMAGE, _IMAGE):
             shape = tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__
             raise ValueError(f"expected crops [N,3,336,336], got {shape}")
@@ -235,7 +266,8 @@ class CLIPVisionTowerB200(nn.Module):
                 x = x.contiguous()
             packed, (w, _) = self._packed_weights(device)
             if train:
-                return _TowerTrainFunction.apply(self, x, packed, self._live_weights(w, train_params, device), *train_params)
+                return _TowerTrainFunction.apply(self, x, packed, self._live_weights(w, train_params, device),
+                                                 wants_gradient_checkpointing(self.vision_model), *train_params)
             ws_bytes = lib.tp_clip_tower_workspace_bytes(n)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
             ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])

@@ -6,10 +6,14 @@ CLIPVisionTowerB200(trainable_layers=K).hidden_states (arm B) against the same s
 Seeded weights at the real shapes (oracle/clip_tower_oracle.py).  Arm A: the oracle's bf16 eager restatement of transformers' tower
 (same rounding points, F.scaled_dot_product_attention), layers 0 .. 22 - K under torch.no_grad(), layers 23 - K .. 22 under autograd
 — what freezing the bottom of CLIPVisionModel gives.  If transformers is importable, arm C is its CLIPVisionModel in bf16 with the same
-layers unfrozen (it runs all 24 layers and keeps every hidden state).  The loss is a fixed weighted sum of hidden states 12 / 16 / 22 / 23
-(those that depend on a trainable layer), so the backward starts from four dense gradients as the projector's input gradients do.
-Alternated rounds, CUDA events around forward + backward, medians; peak memory of one step above what was allocated before it.
-Work per crop is algorithmic (formula below), not measured.
+layers unfrozen (it runs all 24 layers and keeps every hidden state).  Arm D is arm B with gradient checkpointing (the wrapped model's
+``gradient_checkpointing`` switch on: include/tokenpacker_b200_clip_tower_ckpt.h), arm E arm C after ``gradient_checkpointing_enable()``.
+The loss is a fixed weighted sum of hidden states 12 / 16 / 22 / 23 (those that depend on a trainable layer), so the backward starts from
+four dense gradients as the projector's input gradients do.  Alternated rounds, CUDA events around forward + backward, medians; peak
+memory of one step above what was allocated before it.  Work per crop is algorithmic (formula below), not measured.
+
+Before an arm runs, its peak is predicted from the size queries (``predict_bytes``) and compared with torch.cuda.mem_get_info(); an arm
+the prediction rules out is recorded as "does not fit: needs X GB" instead of being run into an out-of-memory error.
 """
 import argparse
 import json
@@ -38,6 +42,28 @@ def step_gflop_per_crop(k, layers=23, t=577, d=1024, f=4096, patches=576, kk=588
     return forward / 1e9, backward / 1e9
 
 
+# Arms without a size query of their own are predicted from ours in the same mode, times the ratio of their peak to ours observed at
+# 64 crops (tools/bench_clip_tower_train_h100.json: eager <= 0.8 - 1.1x, transformers 1.2 - 1.35x); the margin covers allocator slack.
+_PREDICT_SCALE = {"A": 1.1, "B": 1.0, "C": 1.35, "D": 1.0, "E": 1.35}
+_MARGIN = 1.1
+
+
+def predict_bytes(lib, arm, n, k):
+    """Peak bytes of one step above its start: what is kept between forward and backward, plus the larger of the forward's workspace
+    and the backward's workspace with the parameter gradients (16 tensors per layer, 12.6 M elements) and the four outputs' gradients."""
+    outs = 4 * n * 577 * 1024 * 2
+    grads = k * 12_596_224 * 2 + outs
+    if arm in ("D", "E"):
+        kept, fwd, bwd = (lib.tp_clip_tower_ckpt_saved_bytes(n, k), lib.tp_clip_tower_workspace_bytes(n),
+                          lib.tp_clip_tower_ckpt_backward_workspace_bytes(n, k))
+    else:
+        kept, fwd, bwd = (lib.tp_clip_tower_train_saved_bytes(n, k), lib.tp_clip_tower_train_workspace_bytes(n, k),
+                          lib.tp_clip_tower_backward_workspace_bytes(n, k))
+    if arm in ("C", "E"):
+        kept += 25 * n * 577 * 1024 * 2                                # transformers keeps every hidden state
+    return int(_PREDICT_SCALE[arm] * (kept + outs + max(fwd, bwd + grads)))
+
+
 def eager_layer(x, p):
     n = x.shape[0]
     y = F.layer_norm(x, (1024,), p["layer_norm1.weight"], p["layer_norm1.bias"], 1e-5)
@@ -58,9 +84,10 @@ def main():
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs an H100"
     dev = "cuda:0"
-    from tokenpacker_b200 import CLIPVisionTowerB200
+    from tokenpacker_b200 import CLIPVisionTowerB200, _lib
     w = cto.make_weights(23, seed=11, device=dev)
     wb = {k: v.bfloat16() for k, v in w.items()}
+    del w
     n = args.crops
     x = cto.make_images(n, seed=n, device=dev).bfloat16()
     g = torch.Generator(device=dev).manual_seed(5)
@@ -69,7 +96,8 @@ def main():
                          text=True).stdout.strip()
     result = {"bench": "clip_tower_train", "gpu_name_powerlimit_maxsmclock_smclock": smi, "crops": n,
               "arm_a": "oracle bf16 eager restatement under autograd, frozen layers under no_grad",
-              "arm_b": "CLIPVisionTowerB200(trainable_layers=K).hidden_states + backward", "workloads": []}
+              "arm_b": "CLIPVisionTowerB200(trainable_layers=K).hidden_states + backward",
+              "arm_d": "arm B with the wrapped model's gradient_checkpointing switch on", "workloads": []}
     try:
         import transformers
         cfg = transformers.CLIPVisionConfig(hidden_size=1024, intermediate_size=4096, num_attention_heads=16, num_hidden_layers=24,
@@ -78,7 +106,12 @@ def main():
         sd = hf.state_dict()
         sd.update({"vision_model." + k: v for k, v in wb.items()})
         hf.load_state_dict(sd)
+        hf_ckpt = transformers.CLIPVisionModel(cfg).to(dev, torch.bfloat16).train()      # transformers recomputes only in training
+        hf_ckpt.load_state_dict(sd)
+        hf_ckpt.gradient_checkpointing_enable()
+        del sd
         result["arm_c"] = f"transformers {transformers.__version__} CLIPVisionModel bf16 under autograd, same layers unfrozen"
+        result["arm_e"] = "arm C after gradient_checkpointing_enable()"
     except ImportError:
         hf = None
 
@@ -90,6 +123,11 @@ def main():
             if "encoder.layers." in name and int(name.split("encoder.layers.")[1].split(".")[0]) >= first:
                 p.requires_grad_(True)
         ours = CLIPVisionTowerB200(model, trainable_layers=k)
+        model_ckpt = cto.FakeCLIPVisionModel(wb)
+        for name, p in model_ckpt.named_parameters():
+            p.requires_grad_("encoder.layers." in name and int(name.split("encoder.layers.")[1].split(".")[0]) >= first)
+        model_ckpt.gradient_checkpointing = True
+        ours_ckpt = CLIPVisionTowerB200(model_ckpt, trainable_layers=k)
         eager_params = [{key: wb[full].clone().requires_grad_(True) for key, full in cto.layer_keys(i).items()} for i in range(first, 23)]
 
         def loss_of(hs):
@@ -112,18 +150,41 @@ def main():
             for p in model.parameters():
                 p.grad = None
 
+        def run_d():
+            loss_of(ours_ckpt.hidden_states(x)).backward()
+            for p in model_ckpt.parameters():
+                p.grad = None
+
         arms = [("A", run_a), ("B", run_b)]
         if hf is not None:
-            for name, p in hf.named_parameters():
-                p.requires_grad_("encoder.layers." in name and first <= int(name.split("encoder.layers.")[1].split(".")[0]) < 23)
+            for m in (hf, hf_ckpt):
+                for name, p in m.named_parameters():
+                    p.requires_grad_("encoder.layers." in name and first <= int(name.split("encoder.layers.")[1].split(".")[0]) < 23)
 
-            def run_c():
-                hs = hf(pixel_values=x, output_hidden_states=True).hidden_states
-                loss_of([hs[j] for j in cto.OUT_LAYERS]).backward()
-                for p in hf.parameters():
-                    p.grad = None
+            def run_hf(m):
+                def run():
+                    hs = m(pixel_values=x, output_hidden_states=True).hidden_states
+                    loss_of([hs[j] for j in cto.OUT_LAYERS]).backward()
+                    for p in m.parameters():
+                        p.grad = None
+                return run
 
-            arms.append(("C", run_c))
+            arms.append(("C", run_hf(hf)))
+        arms.append(("D", run_d))
+        if hf is not None:
+            arms.append(("E", run_hf(hf_ckpt)))
+        row = {"trainable_layers": k}
+        fitting = []
+        for name, fn in arms:
+            torch.cuda.empty_cache()
+            need = predict_bytes(_lib.lib, name, n, k)
+            free = torch.cuda.mem_get_info()[0]
+            row[name] = {"predicted_bytes": need, "free_bytes_before": int(free)}
+            if need * _MARGIN > free:
+                row[name]["does_not_fit"] = f"does not fit: needs {need / 1e9:.1f} GB"
+            else:
+                fitting.append((name, fn))
+        arms = fitting
         times = {name: [] for name, _ in arms}
         mem = {}
         for name, fn in arms:                                       # warm-up, then the peak memory of one step on its own
@@ -135,6 +196,7 @@ def main():
             fn()
             torch.cuda.synchronize()
             mem[name] = torch.cuda.max_memory_allocated() - base
+            torch.cuda.empty_cache()
         for _ in range(args.rounds):
             for name, fn in arms:
                 s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -144,15 +206,17 @@ def main():
                 torch.cuda.synchronize()
                 times[name].append(s.elapsed_time(e))
         fwd_gf, bwd_gf = step_gflop_per_crop(k)
-        row = {"trainable_layers": k, "gflop_per_crop_forward": round(fwd_gf, 2), "gflop_per_crop_backward": round(bwd_gf, 2)}
+        row.update({"gflop_per_crop_forward": round(fwd_gf, 2), "gflop_per_crop_backward": round(bwd_gf, 2)})
         for name, _ in arms:
             ms = statistics.median(times[name])
-            row[name] = {"ms_median": round(ms, 3), "ms_all": [round(t, 3) for t in times[name]],
-                         "tflops_algorithmic": round((fwd_gf + bwd_gf) * n / ms, 1), "peak_bytes_above_start": int(mem[name])}
-        row["time_B_over_A"] = round(row["B"]["ms_median"] / row["A"]["ms_median"], 3)
-        row["peak_memory_B_over_A"] = round(row["B"]["peak_bytes_above_start"] / row["A"]["peak_bytes_above_start"], 3)
+            row[name].update({"ms_median": round(ms, 3), "ms_all": [round(t, 3) for t in times[name]],
+                              "tflops_algorithmic": round((fwd_gf + bwd_gf) * n / ms, 1), "peak_bytes_above_start": int(mem[name])})
+        for a, b in (("B", "A"), ("D", "B"), ("E", "C"), ("D", "E")):
+            if a in times and b in times:
+                row[f"time_{a}_over_{b}"] = round(row[a]["ms_median"] / row[b]["ms_median"], 3)
+                row[f"peak_memory_{a}_over_{b}"] = round(row[a]["peak_bytes_above_start"] / row[b]["peak_bytes_above_start"], 3)
         result["workloads"].append(row)
-        del ours, model, eager_params
+        del ours, model, ours_ckpt, model_ckpt, eager_params
         torch.cuda.empty_cache()
     line = json.dumps(result)
     print(line)
