@@ -3,8 +3,8 @@
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
 Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
 include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h, include/tokenpacker_b200_clip_tower.h,
-include/tokenpacker_b200_clip_tower_f16.h, include/tokenpacker_b200_clip_tower_train.h and include/tokenpacker_b200_clip_tower_ckpt.h
-one to one.
+include/tokenpacker_b200_clip_tower_f16.h, include/tokenpacker_b200_clip_tower_train.h, include/tokenpacker_b200_clip_tower_ckpt.h and
+include/tokenpacker_b200_clip_tower_embed.h one to one.
 """
 from __future__ import annotations
 
@@ -218,6 +218,23 @@ CLIP_TOWER_CKPT_SIGNATURES = {
 }
 
 
+# the same for include/tokenpacker_b200_clip_tower_embed.h (the whole tower: 23 layers and the embedding stage below them)
+class TpClipTowerEmbedGrads(C.Structure):
+    """tp_clip_tower_embed_grads: one gradient destination per CLIP_TOWER_FIELDS parameter (None: not wanted)."""
+    _fields_ = [(name, C.c_void_p) for name, _ in CLIP_TOWER_FIELDS]
+
+
+CLIP_TOWER_EMBED_SIGNATURES = {
+    "tp_clip_tower_embed_saved_bytes": (C.c_size_t, [C.c_int64]),
+    "tp_clip_tower_forward_train_embed": (C.c_int, [C.c_void_p, C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_int64, C.c_int64, C.c_int,
+                                                    C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                    C.c_size_t, C.c_void_p]),
+    "tp_clip_tower_backward_embed": (C.c_int, [C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_void_p, C.c_int64, C.c_int,
+                                               C.POINTER(C.c_void_p), C.POINTER(TpClipTowerLayerGrads), C.POINTER(TpClipTowerEmbedGrads),
+                                               C.c_void_p, C.c_size_t, C.c_void_p]),
+}
+
+
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -226,7 +243,8 @@ def _load():
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
                                       **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES,
-                                      **CLIP_TOWER_TRAIN_SIGNATURES, **CLIP_TOWER_CKPT_SIGNATURES}.items():
+                                      **CLIP_TOWER_TRAIN_SIGNATURES, **CLIP_TOWER_CKPT_SIGNATURES,
+                                      **CLIP_TOWER_EMBED_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

@@ -24,6 +24,10 @@ parameters of layers 23 - K .. 22 that require grad.  With the projector's ``inp
 When the wrapped model asks for gradient checkpointing (``vision_tower.gradient_checkpointing_enable()``, as the reference's recipes
 do with ``--gradient_checkpointing True``), that training step keeps only each trainable layer's input and derived weights and
 recomputes the rest in the backward (include/tokenpacker_b200_clip_tower_ckpt.h): less memory, more time, the same bits.
+
+``CLIPVisionTowerB200(model, trainable_layers=23, train_embeddings=True)`` trains the whole tower: below the 23 layers, pre_layrnorm, the
+class and position embeddings and the patch embedding get their gradients too (include/tokenpacker_b200_clip_tower_embed.h), with or
+without gradient checkpointing.  That is what the recipes that unfreeze the vision tower (``vision_tower.requires_grad_(True)``) need.
 """
 from __future__ import annotations
 
@@ -46,12 +50,14 @@ _NUM_FN_INPUTS = 5                                      # _TowerTrainFunction's 
 
 class _TowerTrainFunction(torch.autograd.Function):
     """hidden_states 12 / 16 / 22 / 23 with the last K layers under autograd.  Inputs after the first five are the 16 K parameters of
-    the trainable layers, in _lib.CLIP_TOWER_LAYER_FIELDS order, layer 23 - K first.  checkpoint: keep only each trainable layer's
+    the trainable layers, in _lib.CLIP_TOWER_LAYER_FIELDS order, layer 23 - K first; with ``tower.train_embeddings`` (K = 23) the five
+    embedding-stage parameters, in _lib.CLIP_TOWER_FIELDS order, come before them.  checkpoint: keep only each trainable layer's
     checkpoint (include/tokenpacker_b200_clip_tower_ckpt.h) instead of its full saved set; the backward follows the forward's mode."""
 
     @staticmethod
     def forward(ctx, tower, x, packed, w, checkpoint, *params):
         k, n, device = tower.trainable_layers, x.shape[0], x.device
+        embed_saved = None
         outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=torch.bfloat16, device=device) for _ in _OUT_LAYERS)
         if checkpoint:
             forward, name = lib.tp_clip_tower_forward_ckpt, "tp_clip_tower_forward_ckpt"
@@ -64,9 +70,17 @@ class _TowerTrainFunction(torch.autograd.Function):
         ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            check(forward(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), k, ptrs, saved.data_ptr(), saved_bytes, ws.data_ptr(),
-                          ws_bytes, stream), name)
+            if tower.train_embeddings:
+                embed_bytes = lib.tp_clip_tower_embed_saved_bytes(n)
+                embed_saved = torch.empty(embed_bytes, dtype=torch.uint8, device=device)
+                check(lib.tp_clip_tower_forward_train_embed(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), int(checkpoint), ptrs,
+                                                            saved.data_ptr(), saved_bytes, embed_saved.data_ptr(), embed_bytes, ws.data_ptr(),
+                                                            ws_bytes, stream), "tp_clip_tower_forward_train_embed")
+            else:
+                check(forward(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), k, ptrs, saved.data_ptr(), saved_bytes,
+                              ws.data_ptr(), ws_bytes, stream), name)
         ctx.w, ctx.saved, ctx.k, ctx.n, ctx.params, ctx.checkpoint = w, saved, k, n, params, checkpoint
+        ctx.embed_saved = embed_saved
         ctx.set_materialize_grads(False)                # an output nobody used arrives as None, not as a tensor of zeros
         # hidden_states[j] is the output of layer j - 1: below the first trainable layer (23 - k) nothing of it depends on a trainable parameter
         frozen = [o for o, j in zip(outs, _OUT_LAYERS) if j - 1 < _lib.CLIP_TOWER_LAYERS - k]
@@ -80,9 +94,20 @@ class _TowerTrainFunction(torch.autograd.Function):
         d_ptrs = (C.c_void_p * 4)(*[None if g is None else g.data_ptr() for g in d_outs])
         per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
         grads = [torch.empty_like(p) if ctx.needs_input_grad[_NUM_FN_INPUTS + i] else None for i, p in enumerate(ctx.params)]
+        n_top = len(_lib.CLIP_TOWER_FIELDS) if ctx.embed_saved is not None else 0
         g_structs = (_lib.TpClipTowerLayerGrads * k)()
         for t in range(k):
-            g_structs[t] = _lib.TpClipTowerLayerGrads(*[None if g is None else g.data_ptr() for g in grads[t * per:(t + 1) * per]])
+            g_structs[t] = _lib.TpClipTowerLayerGrads(*[None if g is None else g.data_ptr() for g in grads[n_top + t * per:n_top + (t + 1) * per]])
+        if ctx.embed_saved is not None:
+            e_struct = _lib.TpClipTowerEmbedGrads(*[None if g is None else g.data_ptr() for g in grads[:n_top]])
+            ws_bytes = (lib.tp_clip_tower_ckpt_backward_workspace_bytes if ctx.checkpoint else lib.tp_clip_tower_backward_workspace_bytes)(n, k)
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+            with torch.cuda.device(device):
+                stream = torch.cuda.current_stream(device).cuda_stream
+                check(lib.tp_clip_tower_backward_embed(C.byref(ctx.w), ctx.saved.data_ptr(), ctx.embed_saved.data_ptr(), n, int(ctx.checkpoint),
+                                                       d_ptrs, g_structs, C.byref(e_struct), ws.data_ptr(), ws_bytes, stream),
+                      "tp_clip_tower_backward_embed")
+            return (None,) * _NUM_FN_INPUTS + tuple(grads)
         if ctx.checkpoint:
             backward, name, ws_bytes = lib.tp_clip_tower_backward_ckpt, "tp_clip_tower_backward_ckpt", lib.tp_clip_tower_ckpt_backward_workspace_bytes(n, k)
         else:
@@ -130,20 +155,32 @@ class CLIPVisionTowerB200(nn.Module):
     ``invalidate_packed()``.
 
     trainable_layers: K in 0 .. 23, bf16 only.  0 (the default): forward only.  K > 0: encoder layers 23 - K .. 22 are trainable: see
-    ``hidden_states``.  Layers 0 .. 22 - K, the embeddings and pre_layrnorm stay frozen whatever their ``requires_grad`` says: they
-    get no gradient.
+    ``hidden_states``.  Layers 0 .. 22 - K stay frozen whatever their ``requires_grad`` says: they get no gradient; so do the
+    embeddings and pre_layrnorm unless ``train_embeddings``.
+
+    train_embeddings: False (the default) or True, which needs trainable_layers = 23.  True: the embedding stage below layer 0 is
+    trainable as well: the patch embedding, ``class_embedding``, ``position_embedding`` and pre_layrnorm's weight and bias, each of
+    which requires grad gets its gradient.  A step trains when any of these five or of the 23 layers' parameters requires grad, so the
+    embeddings can train with every layer frozen.  To train the embeddings below some frozen layers, keep trainable_layers = 23 and
+    set ``requires_grad=False`` on those layers' parameters: the backward still runs through them (their input gradients), and skips
+    their weight gradients.
 
     Gradient checkpointing has no switch of its own: the tower follows the wrapped model's (``gradient_checkpointing_enable()`` /
     ``_disable()``, see ``wants_gradient_checkpointing``).  Checkpointing trades time for memory and no property of the input decides
     between them, so the choice stays with the switch the model and the recipe that sets it already own; a second option here could
     only disagree with it."""
 
-    def __init__(self, vision_model: nn.Module, dtype: torch.dtype | None = None, trainable_layers: int = 0):
+    def __init__(self, vision_model: nn.Module, dtype: torch.dtype | None = None, trainable_layers: int = 0, train_embeddings: bool = False):
         super().__init__()
         if dtype not in (None, torch.bfloat16, torch.float16):
             raise ValueError(f"CLIPVisionTowerB200 computes in torch.bfloat16 (dtype=None) or torch.float16, not {dtype!r}")
         if not isinstance(trainable_layers, int) or isinstance(trainable_layers, bool) or not 0 <= trainable_layers <= _lib.CLIP_TOWER_LAYERS:
             raise ValueError(f"trainable_layers = {trainable_layers!r}: expected an int in 0 .. {_lib.CLIP_TOWER_LAYERS}")
+        if not isinstance(train_embeddings, bool):
+            raise ValueError(f"train_embeddings = {train_embeddings!r}: expected True or False")
+        if train_embeddings and trainable_layers != _lib.CLIP_TOWER_LAYERS:
+            raise ValueError(f"train_embeddings=True needs trainable_layers={_lib.CLIP_TOWER_LAYERS} (got {trainable_layers}): the embedding stage "
+                             "sits below every layer; freeze layers with requires_grad=False instead")
         if trainable_layers > 0 and dtype == torch.float16:
             raise ValueError("trainable_layers > 0 needs the bf16 tower: no released recipe trains CLIP in fp16 (its gradients underflow "
                              "without loss scaling), so the fp16 tower is forward only")
@@ -159,6 +196,7 @@ class CLIPVisionTowerB200(nn.Module):
         self.vision_model = vision_model
         self.dtype = torch.float16 if dtype == torch.float16 else torch.bfloat16
         self.trainable_layers = trainable_layers
+        self.train_embeddings = train_embeddings
         self._names = names
         self._packed = None
         self._packed_key = None
@@ -182,18 +220,26 @@ class CLIPVisionTowerB200(nn.Module):
         return [named[n] for n in self._names]
 
     def _trainable_params(self):
-        """The 16 K parameters of layers 23 - K .. 22, layer by layer in _lib.CLIP_TOWER_LAYER_FIELDS order."""
+        """The 16 K parameters of layers 23 - K .. 22, layer by layer in _lib.CLIP_TOWER_LAYER_FIELDS order; with train_embeddings, the
+        five embedding-stage parameters (_lib.CLIP_TOWER_FIELDS order) before them."""
+        if self.train_embeddings:
+            return self._params()
         per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
         first = len(_lib.CLIP_TOWER_FIELDS) + (_lib.CLIP_TOWER_LAYERS - self.trainable_layers) * per
         return self._params()[first:] if self.trainable_layers > 0 else []
 
     def _live_weights(self, w, train_params, device):
-        """A copy of the weight struct whose trainable layers point at the live parameters."""
+        """A copy of the weight struct whose trainable layers (and with train_embeddings, embedding stage) point at the live parameters."""
         for p in train_params:
             if p.dtype != torch.bfloat16 or p.device != device or not p.is_contiguous() or p.data_ptr() % 16 != 0:
                 raise ValueError("the trainable layers' parameters are read in place: they must be contiguous, 16-byte aligned bf16 tensors "
                                  "on the crops' device")
         live = _lib.TpClipTowerWeights.from_buffer_copy(w)
+        if self.train_embeddings:
+            n_top = len(_lib.CLIP_TOWER_FIELDS)
+            for (field, _), p in zip(_lib.CLIP_TOWER_FIELDS, train_params[:n_top]):
+                setattr(live, field, p.data_ptr())
+            train_params = train_params[n_top:]
         per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
         first = _lib.CLIP_TOWER_LAYERS - self.trainable_layers
         for t in range(self.trainable_layers):
@@ -243,7 +289,10 @@ class CLIPVisionTowerB200(nn.Module):
         When, in addition, the wrapped model asks for gradient checkpointing (``wants_gradient_checkpointing``, read at every call),
         the step keeps per trainable layer only its input and its derived weights (1.2 MB per crop plus 6.3 MB, against 20.1 MB per
         crop), and the backward recomputes each layer's intermediates before its gradients: the outputs and every gradient have the same
-        bits as without it.  A graph keeps the mode it was built with."""
+        bits as without it.  A graph keeps the mode it was built with.
+        With train_embeddings (trainable_layers = 23), the embedding stage's five parameters count among the trainable ones above: read
+        in place under the same conditions, each that requires grad gets its gradient, and the step keeps in addition the crops' patch
+        rows and the patch embedding's output (1.9 MB per crop), in both modes."""
         if not isinstance(images, torch.Tensor) or images.dim() != 4 or tuple(images.shape[1:]) != (3, _IMAGE, _IMAGE):
             shape = tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__
             raise ValueError(f"expected crops [N,3,336,336], got {shape}")
