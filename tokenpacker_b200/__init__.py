@@ -9,8 +9,9 @@ from . import _lib  # noqa: F401  (fails loudly when the CUDA library is not bui
 from .projector import TokenPackerB200, TokenPacker, build_vision_projector, IdentityMap
 from .hd import Image_Patch, hd_grid, hd_tile, hd_tile_batch, hd_preprocess_batch, hd_plan, hd_assemble, hd_seq_len
 from .clip import clip_preprocess_batch
+from .jpeg import decode_jpeg_batch, jpeg_unsupported
 from .splice import splice_multimodal, splice_plan
 from .tower import CLIPVisionTowerB200
 
 __all__ = ["TokenPackerB200", "TokenPacker", "build_vision_projector", "IdentityMap", "Image_Patch", "hd_grid", "hd_tile", "hd_tile_batch",
-           "hd_preprocess_batch", "hd_plan", "hd_assemble", "hd_seq_len", "clip_preprocess_batch", "splice_multimodal", "splice_plan", "CLIPVisionTowerB200"]
+           "hd_preprocess_batch", "hd_plan", "hd_assemble", "hd_seq_len", "clip_preprocess_batch", "decode_jpeg_batch", "jpeg_unsupported", "splice_multimodal", "splice_plan", "CLIPVisionTowerB200"]

@@ -3,8 +3,8 @@
 There is deliberately no fallback: if the shared library is missing the import fails loudly with the build command.
 Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
 include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h, include/tokenpacker_b200_clip_tower.h,
-include/tokenpacker_b200_clip_tower_f16.h, include/tokenpacker_b200_clip_tower_train.h, include/tokenpacker_b200_clip_tower_ckpt.h and
-include/tokenpacker_b200_clip_tower_embed.h one to one.
+include/tokenpacker_b200_clip_tower_f16.h, include/tokenpacker_b200_clip_tower_train.h, include/tokenpacker_b200_clip_tower_ckpt.h,
+include/tokenpacker_b200_clip_tower_embed.h and include/tokenpacker_b200_jpeg.h one to one.
 """
 from __future__ import annotations
 
@@ -235,6 +235,44 @@ CLIP_TOWER_EMBED_SIGNATURES = {
 }
 
 
+# the same for include/tokenpacker_b200_jpeg.h (baseline JPEG files decoded on the GPU, bit for bit as PIL)
+class TpJpegImage(C.Structure):
+    """tp_jpeg_image: one row of the decode plan."""
+    _fields_ = [(n, C.c_int32) for n in ("reason", "h", "w", "ncomp", "hs", "vs", "mcus_x", "mcus_y", "blocks_per_mcu", "restart",
+                                         "n_segments")] + \
+               [("comp_bx", C.c_int32 * 3), ("comp_by", C.c_int32 * 3), ("reserved", C.c_int32)] + \
+               [(n, C.c_int64) for n in ("scan_offset", "scan_bytes", "unstuffed_offset", "seg_offset", "sub_offset", "sub_capacity",
+                                         "coef_offset", "n_blocks", "block0", "plane_offset", "out_offset", "pixel0")]
+
+
+class TpJpegHuff(C.Structure):
+    _fields_ = [("lookup", C.c_uint16 * 512), ("maxcode", C.c_int32 * 18), ("valoff", C.c_int32 * 18), ("values", C.c_uint8 * 256)]
+
+
+class TpJpegTables(C.Structure):
+    _fields_ = [("dc", TpJpegHuff * 3), ("ac", TpJpegHuff * 3), ("quant", (C.c_uint16 * 64) * 3)]
+
+
+class TpJpegTotals(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("staged_bytes", "output_bytes", "workspace_bytes", "blocks", "pixels")]
+
+
+class TpJpegStatus(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("status", "sync_rounds", "subsequences", "reserved")]
+
+
+TP_JPEG_SUPPORTED = 0
+TP_JPEG_STATUS_OK, TP_JPEG_STATUS_ENTROPY, TP_JPEG_STATUS_RESTART = 0, 1, 2
+JPEG_SIGNATURES = {
+    "tp_jpeg_plan": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int64, C.POINTER(TpJpegImage), C.c_void_p, C.c_void_p,
+                               C.POINTER(TpJpegTotals)]),
+    "tp_jpeg_workspace_bytes": (C.c_size_t, [C.POINTER(TpJpegImage), C.c_int64]),
+    "tp_jpeg_reason_string": (C.c_char_p, [C.c_int]),
+    "tp_jpeg_decode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t,
+                                       C.c_void_p, C.c_void_p]),
+}
+
+
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -244,7 +282,7 @@ def _load():
     for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
                                       **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES,
                                       **CLIP_TOWER_TRAIN_SIGNATURES, **CLIP_TOWER_CKPT_SIGNATURES,
-                                      **CLIP_TOWER_EMBED_SIGNATURES}.items():
+                                      **CLIP_TOWER_EMBED_SIGNATURES, **JPEG_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

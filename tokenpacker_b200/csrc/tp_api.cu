@@ -21,12 +21,14 @@
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"
 #include "../../include/tokenpacker_b200_layers.h"
+#include "../../include/tokenpacker_b200_jpeg.h"
 #include "tp_gemm.cuh"
 #include "tp_kernels.cuh"
 #include "tp_backward.cuh"
 #include "tp_clip_tower.cuh"
 #include "tp_clip_tower_train.cuh"
 #include "tp_clip_tower_embed.cuh"
+#include "tp_jpeg.cuh"
 
 namespace {
 
@@ -1910,3 +1912,4 @@ int tp_hd_fill_separators(void* out, int hidden, const int64_t* sep_rows, int64_
 #include "tp_clip_tower_train.inl"
 #include "tp_clip_tower_ckpt.inl"
 #include "tp_clip_tower_embed.inl"
+#include "tp_jpeg.inl"
