@@ -49,9 +49,10 @@ enum {
 /* what the GPU reports per file (tp_jpeg_status.status) */
 enum {
   TP_JPEG_STATUS_OK = 0,
-  TP_JPEG_STATUS_ENTROPY = 1, /* the entropy-coded data is corrupt or truncated: an invalid code, a run past coefficient 63, bits
+  TP_JPEG_STATUS_ENTROPY = 1, /* the entropy-coded data is corrupt or truncated: an invalid code, bits
                                  read past the end of a restart interval, or an interval with too few blocks */
-  TP_JPEG_STATUS_RESTART = 2  /* the scan has a different number of RSTn markers than its restart interval implies */
+  TP_JPEG_STATUS_RESTART = 2  /* the scan has a different number of RSTn markers than its restart interval implies, or marker k
+                                 (ending interval k) is not RST(k mod 8) */
 };
 
 #define TP_JPEG_SUBSEQUENCE_BYTES 128   /* unit of the parallel Huffman decode */

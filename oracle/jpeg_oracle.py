@@ -79,7 +79,7 @@ def parse(data: bytes) -> dict:
                 counts = list(seg[j + 1:j + 17])
                 vals = list(seg[j + 17:j + 17 + sum(counts)])
                 j += 17 + sum(counts)
-                (ac if tc else dc)[th] = _huff(counts, vals)
+                (ac if tc else dc)[th] = (counts, vals)     # checked and built only if the scan references it, as libjpeg does
         elif m == 0xDD:
             hdr["restart"] = _u16(seg, 0)
         elif m == 0xEE and seg[:5] == b"Adobe":
@@ -107,8 +107,8 @@ def parse(data: bytes) -> dict:
     if len(hdr["scan"]) != nc:
         raise Unsupported("multi-scan")
     hdr["q"] = [q[c["tq"]] for c in hdr["comps"]]
-    hdr["dc"] = [dc[t] for _, t, _ in hdr["scan"]]
-    hdr["ac"] = [ac[t] for _, _, t in hdr["scan"]]
+    hdr["dc"] = [_huff(*dc[t], is_dc=True) for _, t, _ in hdr["scan"]]
+    hdr["ac"] = [_huff(*ac[t], is_dc=False) for _, _, t in hdr["scan"]]
     # scan bytes: up to the first marker that is neither a stuffed 0xFF00 nor RSTn
     j = i
     while True:
@@ -133,20 +133,26 @@ def parse(data: bytes) -> dict:
     return hdr
 
 
-def _huff(counts, vals):
-    """{(length, code): symbol}"""
+def _huff(counts, vals, is_dc):
+    """{(length, code): symbol}.  Refuses the tables libjpeg's jpeg_make_d_derived_tbl refuses: the codes of a length must fit in
+    that many bits and the last of them must not be all ones, and a DC table lists no symbol above 15."""
+    if is_dc and any(v > 15 for v in vals):
+        raise Unsupported("DC Huffman table with a symbol above 15")
     table, code, k = {}, 0, 0
     for ln in range(1, 17):
         for _ in range(counts[ln - 1]):
             table[(ln, code)] = vals[k]
             code += 1
             k += 1
+        if counts[ln - 1] and code >= 1 << ln:
+            raise Unsupported("Huffman table with an all-ones code or too many codes")
         code <<= 1
     return table
 
 
 def unstuff(scan: bytes):
-    """Entropy-coded bytes with stuffing removed, split at RSTn: a list of byte strings, one per restart interval."""
+    """Entropy-coded bytes with stuffing removed, split at RSTn: a list of byte strings, one per restart interval.  Marker k (the
+    one ending interval k) must be RST(k mod 8): libjpeg resynchronises on any other, which this decoder does not restate."""
     segs, cur, i = [], bytearray(), 0
     while i < len(scan):
         b = scan[i]
@@ -157,6 +163,8 @@ def unstuff(scan: bytes):
                 i += 2
                 continue
             if 0xD0 <= n <= 0xD7:
+                if n - 0xD0 != len(segs) % 8:
+                    raise ValueError("restart marker out of sequence")
                 segs.append(bytes(cur))
                 cur = bytearray()
                 i += 2
@@ -222,12 +230,10 @@ def coefficients(hdr: dict):
                     if n == 0:
                         if r != 15:
                             break
-                        k += 16
+                        k += 16                        # a ZRL past 63 ends the block
                         continue
-                    k += r
-                    if k > 63:
-                        raise ValueError("bad AC run")
-                    blk[ZIGZAG[k]] = extend(read(n), n)
+                    k += r                             # a run past 63 stores at 63 (libjpeg's padded jpeg_natural_order)
+                    blk[ZIGZAG[min(k, 63)]] = extend(read(n), n)
                     k += 1
             if pos > nb:
                 raise ValueError("truncated entropy-coded segment")
@@ -280,6 +286,10 @@ def idct_islow(coef, q):
     16-bit (they wrap), as libjpeg-turbo's SIMD dequantisation leaves them."""
     x = _w16(coef.astype(np.int64).reshape(-1, 8, 8) * q.reshape(1, 8, 8))   # [N, row (v), col (u)]
     ws = _idct_1d(x, CONST_BITS - PASS1_BITS)                                  # columns: over rows (axis 1)
+    # the SIMD pass 1 skips the column IDCT of a block whose coefficient rows 1 .. 7 are all zero: every output row is then
+    # row 0 dequantised and shifted left by PASS1_BITS in 16 bits, which wraps where the full pass saturates
+    flat = (coef.reshape(-1, 8, 8)[:, 1:, :] == 0).all(axis=(1, 2))
+    ws[flat] = _w16(x[flat, :1, :] << PASS1_BITS)
     out = _idct_1d(ws.transpose(0, 2, 1), CONST_BITS + PASS1_BITS + 3)         # rows: over columns
     return range_limit(out.transpose(0, 2, 1))
 

@@ -75,7 +75,7 @@ __global__ void __launch_bounds__(kUnstuffThreads) jpeg_unstuff_kernel(const tp_
         } else if (!(prev == 0xFF && (cur == 0x00 || (cur >= 0xD0 && cur <= 0xD7)))) {
           kind[j] = 1;
         }
-        val[j] = static_cast<unsigned char>(cur);
+        val[j] = static_cast<unsigned char>(kind[j] == 2 ? next : cur);    // a marker keeps its number
         cnt.x += kind[j] == 1;
         cnt.y += kind[j] == 2;
       }
@@ -88,6 +88,7 @@ __global__ void __launch_bounds__(kUnstuffThreads) jpeg_unstuff_kernel(const tp_
     for (int j = 0; j < kUnstuffBytesPerThread; ++j) {
       if (kind[j] == 1) dst[o++] = val[j];
       else if (kind[j] == 2) {
+        if ((val[j] & 7) != (r & 7)) status[blockIdx.x].status = TP_JPEG_STATUS_RESTART;   // marker r ends interval r: RST(r mod 8)
         ++r;                                   // interval r starts here
         if (r < im.n_segments) segs[r] = o;
       }
@@ -250,19 +251,20 @@ __device__ __forceinline__ void jpeg_decode_span(const JpegSmem& sm, const tp_jp
       const int rs = jpeg_huff_decode(sm.t.ac[c], br);
       if (rs < 0) { err = true; break; }
       const int r = rs >> 4, s = rs & 15;
+      // as libjpeg decodes them: a ZRL that runs past coefficient 63 ends the block, and a run past 63 stores its value at 63 (through
+      // the padding of jpeg_natural_order); both clamps also keep the zero fill and sm.zz inside their 64 entries
       if (s == 0) {
-        const int kend = r == 15 ? k + 16 : 64;
-        if (kend > 64) { err = true; break; }
+        const int kend = r == 15 && k + 16 < 64 ? k + 16 : 64;
         if (blk) for (int j = k; j < kend; ++j) blk[sm.zz[j]] = 0;
         k = kend;
       } else {
-        if (k + r > 63) { err = true; break; }
+        const int at = k + r < 63 ? k + r : 63;
         const int v = jpeg_extend(br.get(s), s);
         if (blk) {
-          for (int j = k; j < k + r; ++j) blk[sm.zz[j]] = 0;
-          blk[sm.zz[k + r]] = static_cast<int16_t>(v);
+          for (int j = k; j < at; ++j) blk[sm.zz[j]] = 0;
+          blk[sm.zz[at]] = static_cast<int16_t>(v);
         }
-        k += r + 1;
+        k = at + 1;
       }
       // checked before the block is closed, so that the error names the block whose code or value read the zeros past the end
       if (br.pos > sub.seg_end) { err = true; break; }
@@ -494,6 +496,7 @@ __global__ void __launch_bounds__(kIdctThreads) jpeg_idct_kernel(const tp_jpeg_i
                                                                   const tp_jpeg_tables* __restrict__ tables, uint8_t* ws,
                                                                   long long total_blocks) {
   __shared__ int sblk[kIdctThreads / 8][64];
+  __shared__ int snz[kIdctThreads];                 // per thread: its coefficient row has a nonzero
   const long long g = static_cast<long long>(blockIdx.x) * (kIdctThreads / 8) + threadIdx.x / 8;
   const int r = threadIdx.x & 7;
   int* s = sblk[threadIdx.x / 8];
@@ -516,9 +519,18 @@ __global__ void __launch_bounds__(kIdctThreads) jpeg_idct_kernel(const tp_jpeg_i
   const uint16_t* q = tables[img].quant[c] + r * 8;
 #pragma unroll
   for (int j = 0; j < 8; ++j) s[r * 8 + j] = jpeg_w16(static_cast<int>(cv[j]) * static_cast<int>(q[j]));
+  snz[threadIdx.x] = (raw.x | raw.y | raw.z | raw.w) != 0;
   __syncwarp();
   int o[8];
-  jpeg_idct_1d(s + r, 8, kConstBits - kPass1Bits, o);                 // pass 1: column r
+  const int* nz = snz + (threadIdx.x & ~7);
+  if ((nz[1] | nz[2] | nz[3] | nz[4] | nz[5] | nz[6] | nz[7]) == 0) {
+    // the SIMD pass 1 skips a block whose coefficient rows 1 .. 7 are all zero: each output is row 0 dequantised and shifted left by
+    // PASS1_BITS in 16 bits, which wraps where the full pass saturates
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] = jpeg_w16(s[r] * (1 << kPass1Bits));
+  } else {
+    jpeg_idct_1d(s + r, 8, kConstBits - kPass1Bits, o);               // pass 1: column r
+  }
 #pragma unroll
   for (int j = 0; j < 8; ++j) s[j * 8 + r] = o[j];
   __syncwarp();
