@@ -311,8 +311,12 @@ def test_one_layer_stage_by_stage(hooks, tower):
     """Layer 1 alone on a workspace poisoned with 0xFF bytes (0xFFFF is NaN in f16 too): every stage against fp64 of that stage computed
     from the f16 values the kernels stored before it.  q is scaled by 1/8 after its bias with one rounding (the packed f16 weights are
     unscaled)."""
+    _one_layer_stages(hooks, tower, 2)
+
+
+def _one_layer_stages(hooks, tower, n):
+    """the stages of test_one_layer_stage_by_stage over n crops (tests/test_clip_tower_batches_gpu.py runs the other plans' n)"""
     w, _, t = tower
-    n = 2
     images = cto.make_images(n, seed=21, device=DEV).half()
     with torch.no_grad():
         x = cto.forward(w, images.float(), 1, torch.float64)[1].half().reshape(n * 577, 1024).contiguous()

@@ -219,8 +219,12 @@ def _ln_ref(x, gamma, beta):
 def test_one_layer_stage_by_stage(hooks, tower):
     """Layer 1 alone (its input, hidden_states[1], carries the outlier channels in the outlier variant) on a workspace poisoned with
     NaN: every stage against fp64 of that stage computed from the bf16 values the kernels stored before it."""
+    _one_layer_stages(hooks, tower, 2)
+
+
+def _one_layer_stages(hooks, tower, n):
+    """the stages of test_one_layer_stage_by_stage over n crops (tests/test_clip_tower_batches_gpu.py runs the other plans' n)"""
     w, t = tower
-    n = 2
     images = cto.make_images(n, seed=21, device=DEV).bfloat16()
     with torch.no_grad():
         x = cto.forward(w, images.float(), 1, torch.float64)[1].bfloat16().reshape(n * 577, 1024).contiguous()
