@@ -92,4 +92,20 @@ TP_API int tpc_mixed_precision(int how) {
   return build_pair_group(items, 2, 132, nullptr, &b);
 }
 
+// The embedding stage of tp_clip_tower_forward_f16 alone (run_clip_embed) up to step last_step, as tpc_embed (tp_clip_tower_hooks.cu):
+// crops_dtype TP_CLIP_CROPS_BF16 (converted to f16 rows by im2col) or TP_CLIP_CROPS_F16 (read as they are); offsets from tpc_embed_offsets
+TP_API int tpc_embed_f16(const void* packed, const tp_clip_tower_weights* w, const void* crops, int crops_dtype, int64_t n,
+                         int64_t crop_stride, void* workspace, size_t workspace_bytes, int last_step, void* stream) {
+  if (packed == nullptr || w == nullptr || !clip_weights_complete(w) || crops == nullptr || workspace == nullptr || n <= 0 ||
+      (crops_dtype != TP_CLIP_CROPS_BF16 && crops_dtype != TP_CLIP_CROPS_F16) || crop_stride < 3ll * kClipImage * kClipImage ||
+      last_step < 1 || last_step > 3)
+    return TP_ERR_INVALID_ARGUMENT;
+  const ClipWorkLayout WL = clip_work_layout(n);
+  if (workspace_bytes < WL.total) return TP_ERR_WORKSPACE_TOO_SMALL;
+  DeviceInfo dev;
+  TP_TRY(device_info(&dev));
+  return run_clip_embed(static_cast<const uint8_t*>(packed), w, crops, crops_dtype, n, crop_stride, static_cast<uint8_t*>(workspace), WL,
+                        dev.sms, static_cast<cudaStream_t>(stream), true, nullptr, last_step);
+}
+
 }  // extern "C"

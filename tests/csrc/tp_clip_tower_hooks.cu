@@ -1,6 +1,7 @@
 // Test-only entry points into the CLIP tower's kernels (libtokenpacker_b200_clip_tower_hooks.so, loaded by
-// tests/test_clip_tower_gpu.py; never by the package): the product translation unit plus the tpc_* functions below, which launch the
-// same kernels and GEMM items tp_clip_tower_forward launches.  Conventions as in include/tokenpacker_b200.h.
+// tests/test_clip_tower_gpu.py and tests/test_clip_tower_forward_stages_gpu.py; never by the package): the product translation unit plus
+// the tpc_* functions below, which launch the same kernels and GEMM items tp_clip_tower_forward launches.  Conventions as in
+// include/tokenpacker_b200.h.
 #include "../../tokenpacker_b200/csrc/tp_api.cu"
 
 extern "C" {
@@ -61,6 +62,51 @@ TP_API int tpc_layer(const void* packed, const tp_clip_tower_weights* w, int lay
   int* flags = reinterpret_cast<int*>(W + WL.flags);
   TP_CUDA(cudaMemsetAsync(flags, 0, static_cast<size_t>(WL.flags_per_layer) * 4, stream));
   return run_clip_layer(static_cast<const uint8_t*>(packed), w, layer, x, x_out, W, WL, n, flags, dev.sms, stream);
+}
+
+// Byte offsets inside the workspace of a tp_clip_tower_forward(_f16) call over n crops for the embedding stage: h (the im2col patch rows,
+// [576 n, 592]), xa (hidden_states[0], [577 n, 1024]); out[2] = the workspace size.
+TP_API int tpc_embed_offsets(int64_t n, int64_t* out) {
+  if (n <= 0 || out == nullptr) return TP_ERR_INVALID_ARGUMENT;
+  const ClipWorkLayout L = clip_work_layout(n);
+  const size_t o[3] = {L.h, L.xa, L.total};
+  for (int i = 0; i < 3; ++i) out[i] = static_cast<int64_t>(o[i]);
+  return TP_OK;
+}
+
+// The embedding stage of tp_clip_tower_forward alone (run_clip_embed) up to step last_step (1 = im2col, 2 = + the patch GEMM, 3 = +
+// embeddings and pre_layrnorm), on the caller's workspace.  crops_dtype and crop_stride as in the C ABI (bf16 crops only here).
+TP_API int tpc_embed(const void* packed, const tp_clip_tower_weights* w, const void* crops, int crops_dtype, int64_t n, int64_t crop_stride,
+                     void* workspace, size_t workspace_bytes, int last_step, void* stream) {
+  if (packed == nullptr || w == nullptr || !clip_weights_complete(w) || crops == nullptr || workspace == nullptr || n <= 0 ||
+      crops_dtype != TP_CLIP_CROPS_BF16 || crop_stride < 3ll * kClipImage * kClipImage || last_step < 1 || last_step > 3)
+    return TP_ERR_INVALID_ARGUMENT;
+  const ClipWorkLayout WL = clip_work_layout(n);
+  if (workspace_bytes < WL.total) return TP_ERR_WORKSPACE_TOO_SMALL;
+  DeviceInfo dev;
+  TP_TRY(device_info(&dev));
+  return run_clip_embed(static_cast<const uint8_t*>(packed), w, crops, crops_dtype, n, crop_stride, static_cast<uint8_t*>(workspace), WL,
+                        dev.sms, static_cast<cudaStream_t>(stream), false, nullptr, last_step);
+}
+
+// y [rows, 1024] = LayerNorm(x) gamma + beta, the tower's launch_clip_ln: x_kind 0 = x has the storage type, 1 = x is fp32; f16 = 0: bf16
+// storage (layer_norm1: bf16 -> bf16, layer_norm2: fp32 -> bf16), 1: f16 storage (f16 -> f16, fp32 -> f16)
+TP_API int tpc_layernorm(const void* x, int x_kind, int64_t rows, const void* gamma, const void* beta, void* y, int f16, void* stream_) {
+  if (x == nullptr || gamma == nullptr || beta == nullptr || y == nullptr || rows <= 0 || (x_kind != 0 && x_kind != 1) || (f16 != 0 && f16 != 1))
+    return TP_ERR_INVALID_ARGUMENT;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (f16) return x_kind ? launch_clip_ln<float, __half>(x, rows, gamma, beta, y, stream) : launch_clip_ln<__half, __half>(x, rows, gamma, beta, y, stream);
+  return x_kind ? launch_clip_ln<float>(x, rows, gamma, beta, y, stream) : launch_clip_ln<__nv_bfloat16>(x, rows, gamma, beta, y, stream);
+}
+
+// The fields of the packed derived weights' layout (tp_clip_tower_pack_weights / _f16), in bytes: patch_w, layer0, layer_bytes, and
+// inside a layer's block w_qkv, b_qkv, b_o, b_fc1, b_fc2; out[8] = the total
+TP_API int tpc_packed_layout(int64_t* out) {
+  if (out == nullptr) return TP_ERR_INVALID_ARGUMENT;
+  const ClipPackedLayout L = clip_packed_layout();
+  const size_t o[9] = {L.patch_w, L.layer0, L.layer_bytes, L.w_qkv, L.b_qkv, L.b_o, L.b_fc1, L.b_fc2, L.total};
+  for (int i = 0; i < 9; ++i) out[i] = static_cast<int64_t>(o[i]);
+  return TP_OK;
 }
 
 }  // extern "C"

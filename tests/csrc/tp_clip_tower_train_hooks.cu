@@ -80,4 +80,10 @@ TP_API int tptt_layer_backward(const tp_clip_tower_weights* w, int layer, const 
                                  static_cast<uint8_t*>(ws), B, n, dev.sms, static_cast<cudaStream_t>(stream), last_step);
 }
 
+// z = bf16(z32), h = bf16(quick_gelu(z32)) over n elements (a multiple of 8): the training forward's clip_quick_gelu_fwd_kernel launch
+TP_API int tptt_quick_gelu_fwd(const float* z32, void* z, void* h, int64_t n, void* stream) {
+  if (z32 == nullptr || z == nullptr || h == nullptr || n <= 0 || n % 8 != 0) return TP_ERR_INVALID_ARGUMENT;
+  return launch_clip_quick_gelu_fwd(z32, z, h, n, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

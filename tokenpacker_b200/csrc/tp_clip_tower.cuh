@@ -289,7 +289,8 @@ clip_attn_kernel(const __grid_constant__ CUtensorMap tmap_qkv, T* __restrict__ c
 }
 
 // The q third of the packed [3072, 1024] qkv weight and its fp32 bias times 1/8 (exact: a power of two in bf16, whose exponent range is
-// fp32's; the f16 tower applies 1/8 as the q GEMM's alpha instead, since weights below 2^-11 would lose bits as f16 subnormals)
+// fp32's, except that weights below 2^-123 become bf16 subnormals and round once to nearest even; the f16 tower applies 1/8 as the q
+// GEMM's alpha instead, since weights below 2^-11 would lose bits as f16 subnormals)
 __global__ void clip_scale_q_kernel(__nv_bfloat16* __restrict__ w, float* __restrict__ bias) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < 1024 * 1024) w[i] = __float2bfloat16_rn(__bfloat162float(w[i]) * 0.125f);

@@ -35,10 +35,11 @@ __global__ void __launch_bounds__(256) clip_quick_gelu_fwd_kernel(const float* _
 }
 
 // d/dz [z sigmoid(1.702 z)] = s (1 + 1.702 z (1 - s)), s = sigmoid(1.702 z).  Large |z|: exp overflows to +inf -> s = 0 -> 0; exp
-// underflows to 0 -> s = 1 -> 1; (1 - s) z is formed first so that no inf * 0 appears for any finite z.
+// underflows to 0 -> s = 1 -> 1; (1 - s) z is formed first so that no inf * 0 appears for any finite z.  Below z = -2e38, 1.702 z itself
+// overflows to -inf inside the fma and 0 * -inf would be NaN: (1 - s) z is clamped at -1e38 (s = 0 there already, so no other z changes).
 __device__ __forceinline__ float quick_gelu_grad(float z) {
   const float s = 1.0f / (1.0f + __expf(-1.702f * z));
-  return s * fmaf(1.702f, (1.0f - s) * z, 1.0f);
+  return s * fmaf(1.702f, fmaxf((1.0f - s) * z, -1e38f), 1.0f);
 }
 
 // gelu_bwd_colsum_kernel (tp_backward.cuh) for quick_gelu: dz = dh quick_gelu'(z) in place over dh, fused with the first stage of fc1's
