@@ -15,10 +15,12 @@
 //                        CLIP layers side by side along K), grouped launches and the peer (all-gather) stores.
 //
 // CTA = 384 threads, persistent over output tiles:
-//   warps 0-7   two MMA + epilogue warpgroups, one per column half of the tile: wgmma m64nNk16 over the CTA's 128 rows (two
-//               64-row blocks, 2 x N/2 fp32 accumulators per thread), then the epilogue on the same registers: each warp turns its
-//               fragments into thread == output row form through a 2 KiB shared-memory transpose (32 columns at a time), fused
-//               per-row / per-column math, swizzled shared-memory slabs (16-byte stores) or direct 16-byte global stores
+//   warps 0-7   two MMA + epilogue warpgroups, one per 64-row block of the CTA's 128 rows: one wgmma m64nNk16 per k16 step over
+//               the whole N-column tile (N/2 fp32 accumulators per thread), so each warpgroup reads its A block once and the B tile
+//               once per k-step; then the epilogue on the same registers: each warp turns its fragments into thread == output row
+//               form (lanes 0-15: column half 0, lanes 16-31: column half 1 of the warp's 16 rows) through a 2 KiB shared-memory
+//               transpose (32 columns at a time), fused per-row / per-column math, swizzled shared-memory slabs (16-byte stores)
+//               or direct 16-byte global stores
 //   warps 8, 9  store warps of the pair kernel (one per column half): wait for a finished slab on an mbarrier, issue its TMA
 //               store(s), hand the buffer back, and — for GEMMs that other GEMMs of the same launch depend on — publish each
 //               finished tile to a global counter.  The epilogue warps never wait for a store.
@@ -34,7 +36,7 @@
 //   v = v + R[r, c]                              residual add (bf16 operand read from global memory)
 //   v = gelu_erf(v)  |  v = quick_gelu(v)        exact erf GELU (nn.GELU default) | x sigmoid(1.702 x) (CLIP)
 //   v = alpha * v                                1/sqrt(head_dim) query scaling
-//   y = bf16(v);  stats_out[r][slot] = (mean, M2) of y over this warp's 128 columns  -> next LayerNorm fold (deterministic:
+//   y = bf16(v);  stats_out[r][slot] = (mean, M2) of y over this thread's 128 columns -> next LayerNorm fold (deterministic:
 //                                                one slot per 128-column block, combined Chan-style in fixed order by the consumer)
 //   C[dst_row(r), c] = y                         optional segment scatter (HD packed output)
 #pragma once
@@ -82,8 +84,8 @@ constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;     // 64 bf16 = 128 bytes = one swizzle-128B row
 constexpr int kUmmaK = 16;
 constexpr int kGemmThreads = 384;
-// Warp roles: warps 0-7 are the two MMA + epilogue warpgroups (warpgroup = column half of the tile, warp % 4 = "quarter": the
-// 16 + 16 rows of each 64-row block its wgmma fragments hold), warps 8-11 the producer / store warpgroup.
+// Warp roles: warps 0-7 are the two MMA + epilogue warpgroups (warpgroup = 64-row block of the CTA's 128 rows, warp % 4 =
+// "quarter": the 16 rows of that block its wgmma fragments hold), warps 8-11 the producer / store warpgroup.
 constexpr int kEpiWarp0 = 0;
 constexpr int kTmaWarp = 10;
 constexpr int kStoreWarp0 = 8;      // pair kernel: warps 8 and 9 issue the TMA stores of column half 0 / 1
@@ -95,16 +97,25 @@ constexpr uint32_t kAuxRegs = 72;
 constexpr int kScratchBytesPerWarp = 32 * 16 * 4;     // accumulator transpose: 32 rows x 16 fp32 columns
 constexpr int kScratchBytes = kNumEpiWarps * kScratchBytesPerWarp;
 
-// Tile row of epilogue thread (quarter, lane): the rows whose wgmma fragments warp `quarter` of a warpgroup holds — 16 of each
-// 64-row block — so the fragment -> row transpose never leaves the warp.  Windows of 4 or 16 consecutive rows stay inside 16
-// consecutive lanes.
-__device__ __forceinline__ int epi_row(int quarter, uint32_t lane) {
+// Pair kernel: tile row of epilogue thread (warpgroup wg, quarter, lane): the 16 rows whose wgmma fragments warp `quarter` of
+// warpgroup wg holds, once for each column half (lanes 0-15: half 0, lanes 16-31: half 1: epi_half), so the fragment -> row
+// transpose never leaves the warp.  Windows of 4 or 16 consecutive rows stay inside 16 consecutive lanes.
+__device__ __forceinline__ int epi_row(int wg, int quarter, uint32_t lane) {
+  return 64 * wg + 16 * quarter + static_cast<int>(lane & 15u);
+}
+__device__ __forceinline__ int epi_half(uint32_t lane) { return static_cast<int>(lane >> 4); }
+
+// One-CTA kernel (warpgroup = column half): tile row of epilogue thread (quarter, lane): the 16 rows of each 64-row block whose
+// fragments warp `quarter` holds, lanes 0-15 in block 0 and lanes 16-31 in block 1.
+__device__ __forceinline__ int epi_row_1cta(int quarter, uint32_t lane) {
   return 16 * quarter + static_cast<int>(lane & 15u) + 64 * static_cast<int>(lane >> 4);
 }
 
-// 32 accumulator columns [32 chunk, +32) of this warp's 32 rows (epi_row order) into r: each thread gets its own row.  The two
-// 64-row blocks' fragments go through the warp's scratch, 16 columns at a time, XOR-swizzled so that both the 8-byte fragment
-// stores and the 16-byte row loads are free of bank conflicts.  `chunk` must be a compile-time constant after unrolling.
+// 32 accumulator columns [32 chunk, +32) of each of the warp's two fragment parts into r: lane l gets row l & 15 of part l >> 4.
+// acc[h] is part h: in the pair kernel the column-half-h registers of the m64n256 fragment (registers 64 h ...), in the one-CTA
+// kernel the fragment of 64-row block h.  Both parts go through the warp's scratch, 16 columns at a time, XOR-swizzled so that
+// both the 8-byte fragment stores and the 16-byte row loads are free of bank conflicts.  `chunk` must be a compile-time constant
+// after unrolling.
 __device__ __forceinline__ uint32_t scratch_swz(uint32_t row) { return (((row >> 1) & 1u) << 1) | ((row >> 2) & 1u); }
 
 template <int kAccN>
@@ -115,15 +126,15 @@ __device__ __forceinline__ void acc_chunk(const float (&acc)[2][kAccN], int chun
   for (int t = 0; t < 2; ++t) {
     __syncwarp();                                      // the previous reads of the scratch are done
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb)
+    for (int ch = 0; ch < 2; ++ch)
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int jj = 0; jj < 2; ++jj) {
           const int i = (chunk * 4 + t * 2 + jj) * 4 + 2 * h;
-          const uint32_t row = g + 8u * h + 16u * mb;
+          const uint32_t row = g + 8u * h + 16u * ch;
           const uint32_t unit = ((2u * jj) + (q >> 1)) ^ scratch_swz(row);
-          sts_f2(scratch + row * 64u + unit * 16u + (q & 1u) * 8u, acc[mb][i], acc[mb][i + 1]);
+          sts_f2(scratch + row * 64u + unit * 16u + (q & 1u) * 8u, acc[ch][i], acc[ch][i + 1]);
         }
     __syncwarp();
 #pragma unroll
@@ -137,20 +148,23 @@ __device__ __forceinline__ void acc_chunk(const float (&acc)[2][kAccN], int chun
   }
 }
 
-// One warpgroup's MMAs for a tile: the CTA's 128 rows of A (two 64-row blocks) x kN columns of B starting `b_off` bytes into
-// the stage's B tile, over n_kb k-blocks of the ring.  A stage is released (one arrive per warp on empty_bar) once the wgmmas
-// reading it have retired; one k-block of wgmmas stays in flight while the next one is issued.
-template <int kN, int kTransA, int kTransB, bool kF16 = false>
-__device__ __forceinline__ void mma_tile(float (&acc)[2][kN / 2], const uint8_t* smem, int stage_bytes, int a_bytes, int b_off,
+// One warpgroup's MMAs for a tile: kRowBlocks 64-row blocks of A starting `a_off` bytes into the stage x kN rows of B starting
+// `b_off` bytes into it, over n_kb k-blocks of the ring: per k16 step one m64nNk16 per row block.  The pair kernel: one row block
+// (its warpgroup's) x the whole 256-row B tile, m64n256.  The one-CTA kernel: both row blocks x its warpgroup's column half.
+// A stage is released (one arrive per warp on empty_bar) once the wgmmas reading it have retired; one k-block of wgmmas stays
+// in flight while the next one is issued.
+template <int kN, int kRowBlocks, int kTransA, int kTransB, bool kF16 = false>
+__device__ __forceinline__ void mma_tile(float (&acc)[2][kN * kRowBlocks / 4], const uint8_t* smem, int stage_bytes, int a_off, int b_off,
                                          uint64_t* full_bar, uint64_t* empty_bar, int n_stages, int& stage, uint32_t& phase, int n_kb) {
-  static_assert(kN == 64 || kN == 128, "wgmma N");
+  static_assert(kN == 64 || kN == 128 || kN == 256, "wgmma N");
+  float (&d)[kRowBlocks][kN / 2] = reinterpret_cast<float (&)[kRowBlocks][kN / 2]>(acc);   // per row block: its fragment, wgmma order
   int prev = -1;
   for (int kb = 0; kb < n_kb; ++kb) {
     mbar_wait(&full_bar[stage], phase);         // TMA bytes have landed
-    const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-    const uint32_t sb = sa + static_cast<uint32_t>(a_bytes + b_off);
+    const uint32_t sa = smem_u32(smem + stage * stage_bytes) + static_cast<uint32_t>(a_off);
+    const uint32_t sb = smem_u32(smem + stage * stage_bytes) + static_cast<uint32_t>(b_off);
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb) fence_regs(acc[mb]);
+    for (int mb = 0; mb < kRowBlocks; ++mb) fence_regs(d[mb]);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < kBlockK / kUmmaK; ++k) {
@@ -160,17 +174,18 @@ __device__ __forceinline__ void mma_tile(float (&acc)[2][kN / 2], const uint8_t*
                                   : make_smem_desc_kmajor_sw128(sb) + static_cast<uint64_t>(k * 2);
       const uint32_t accumulate = static_cast<uint32_t>((kb | k) != 0);
 #pragma unroll
-      for (int mb = 0; mb < 2; ++mb) {
+      for (int mb = 0; mb < kRowBlocks; ++mb) {
         const uint32_t sam = sa + static_cast<uint32_t>(mb * 8192);
         const uint64_t da = kTransA ? make_smem_desc_mnmajor_sw128(sam, 8192) + static_cast<uint64_t>(k * 128)
                                     : make_smem_desc_kmajor_sw128(sam) + static_cast<uint64_t>(k * 2);
-        if constexpr (kN == 128) wgmma_m64n128<kTransA, kTransB, kF16>(acc[mb], da, db, accumulate);
-        else wgmma_m64n64<kTransA, kTransB, kF16>(acc[mb], da, db, accumulate);
+        if constexpr (kN == 256) wgmma_m64n256<kTransA, kTransB, kF16>(d[mb], da, db, accumulate);
+        else if constexpr (kN == 128) wgmma_m64n128<kTransA, kTransB, kF16>(d[mb], da, db, accumulate);
+        else wgmma_m64n64<kTransA, kTransB, kF16>(d[mb], da, db, accumulate);
       }
     }
     wgmma_commit();
 #pragma unroll
-    for (int mb = 0; mb < 2; ++mb) fence_regs(acc[mb]);
+    for (int mb = 0; mb < kRowBlocks; ++mb) fence_regs(d[mb]);
     wgmma_wait<1>();                                   // the previous k-block's wgmmas have retired
     if (prev >= 0) {
       __syncwarp();
@@ -181,7 +196,7 @@ __device__ __forceinline__ void mma_tile(float (&acc)[2][kN / 2], const uint8_t*
   }
   wgmma_wait<0>();
 #pragma unroll
-  for (int mb = 0; mb < 2; ++mb) fence_regs(acc[mb]);
+  for (int mb = 0; mb < kRowBlocks; ++mb) fence_regs(d[mb]);
   if (prev >= 0) {
     __syncwarp();
     if (lane_id() == 0) mbar_arrive(&empty_bar[prev]);
@@ -190,14 +205,16 @@ __device__ __forceinline__ void mma_tile(float (&acc)[2][kN / 2], const uint8_t*
 
 // ------------------------------------------------------------------------------------------------
 // Shared epilogue for one 128-row x kTileN-column accumulator tile held in the registers of the CTA's two MMA warpgroups.
-//   acc      : this warpgroup's (= column half's) wgmma accumulators
+//   acc      : this warpgroup's (= 64-row block's) wgmma accumulators, [column half][fragment registers of the half]
 //   scratch  : shared address of this warp's transpose scratch (kScratchBytesPerWarp)
-//   row      : global output row of this thread (tile row epi_row(quarter, lane))
+//   row      : global output row of this thread (tile row rloc = epi_row(wg, quarter, lane))
 //   col_tile0: global column of the tile's first column
-//   s_col    : shared staging for this tile's col_a / col_b slices, [2][kTileN] floats (already filled + synced)
+//   half     : the column half this thread owns (epi_half(lane))
+//   s_col    : shared staging for this tile's col_a / col_b slices, col_slot layout (already filled + synced)
 // ------------------------------------------------------------------------------------------------
-// Output staging for TMA stores: each column half of the tile (4 warps) owns two 16 KiB buffers holding a 128-row x 64-col
-// slab in the 128B-swizzled layout; a slab is written with conflict-free 16-byte st.shared, then ONE thread hands it
+// Output staging for TMA stores: each column half of the tile owns two 16 KiB buffers holding a 128-row x 64-col slab in the
+// 128B-swizzled layout, 16 rows of it from each of the 8 epilogue warps (the 16 lanes of the warp that own that half); a slab is
+// written with conflict-free 16-byte st.shared, then ONE thread hands it
 // to the TMA unit (full 128-byte row segments instead of 16-byte scattered stores: less L1/L2 work and less power).
 constexpr int kMaxPeers = 8;
 // Fused all-gather: tensor maps of the SAME output slot in every peer GPU's gathered buffer (peer-mapped over NVLink);
@@ -212,7 +229,7 @@ struct PeerStores {
 
 struct OutStage {
   uint8_t* buf;              // this half's 2 x 16 KiB staging buffers (nullptr: direct 16-byte global stores)
-  uint64_t* full_bar;        // [2] slab written (count 4: one arrive per epilogue warp of the half) -> store warp
+  uint64_t* full_bar;        // [2] slab written (count 8: one arrive per epilogue warp, from its lanes of the half) -> store warp
   uint64_t* empty_bar;       // [2] slab's TMA store has finished reading the buffer (count 1, store warp) -> epilogue warps
   uint32_t slab_seq;         // running slab number of this half (buffer = seq % 2, mbarrier phase = seq / 2)
 };
@@ -221,6 +238,13 @@ constexpr int kSlabCols = 64;
 constexpr int kSlabRowBytes = kSlabCols * 2;
 constexpr int kChunksPerSlab = kSlabCols / 32;
 constexpr int kOutSlabBytes = 128 * kSlabRowBytes;
+
+// Shared staging of a tile's per-column vectors: [col_a | col_b] x [column half 0 | kColPad | column half 1 | kColPad] floats.
+// In the pair kernel the two halves of a warp read the same offset of their half at once; the padding puts those two addresses
+// in different banks.
+constexpr int kColPad = 4;
+template <int kTileN>
+__host__ __device__ constexpr int col_slot(int vec, int c) { return vec * (kTileN + 2 * kColPad) + c + (c >= kTileN / 2 ? kColPad : 0); }
 
 // raster row (crop n, token row tr, token column tc) -> window-major row (crop n, window (hb, wb), key (hi, wi)) for windows of s x s
 __device__ __forceinline__ long long window_major_row(long long row, int s) {
@@ -252,12 +276,16 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
 // kTower: the CLIP tower's instantiations (bias, bf16 or fp32 residual add, quick_gelu, alpha, fp32 output) — and none of the
 // projector's LayerNorm fold, row statistics, dual / window-major outputs, so that neither set of instantiations carries the other's registers.
 // kF16 (tower only): the same with an f16 residual and f16 output (one __floats2half2_rn rounding).
-template <int kTileN, bool kTower = false, bool kF16 = false>
+// kSubPairs: packed column pairs (2 columns each) that go through every step together: each run-time option is ONE warp-uniform
+// branch around a basic block of kSubPairs independent dependency chains for the scheduler to interleave (more chains, more
+// registers).  8 in the one-CTA kernel; 4 in the pair kernel, where the column half is a per-lane value and 8 chains spill at
+// the 216-register limit.
+template <int kTileN, bool kTower = false, bool kF16 = false, int kSubPairs = 8>
 __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int N, const float (&acc)[2][kTileN / 4], uint32_t scratch,
-                                              int row, int col_tile0, int quarter, int half, const float* s_col, const OutStage& out,
+                                              int row, int rloc, int col_tile0, int half, const float* s_col, const OutStage& out,
                                               long long c_extra = 0) {
-  constexpr int kColsPerWarp = kTileN / 2;
-  constexpr int kChunks = kColsPerWarp / 32;
+  constexpr int kColsPerHalf = kTileN / 2;
+  constexpr int kChunks = kColsPerHalf / 32;
   const bool ln_fold = !kTower && ep.col_a != nullptr;
   const bool row_ok = row < M;
   float mu = 0.f, rstd = 1.f;
@@ -276,7 +304,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
   }
   __nv_bfloat16* c_row = static_cast<__nv_bfloat16*>(ep.c) + dst_row * ep.ldc;     // 16-bit elements (bf16 or f16: stored as raw bits)
   float* c_row32 = reinterpret_cast<float*>(ep.c) + c_extra + dst_row * ep.ldc;     // out_f32 only (c_extra: split-K slice)
-  const uint32_t sa_addr = smem_u32(s_col + half * kColsPerWarp), sb_addr = smem_u32(s_col + kTileN + half * kColsPerWarp);
+  const uint32_t sa_addr = smem_u32(s_col + col_slot<kTileN>(0, half * kColsPerHalf));
+  const uint32_t sb_addr = smem_u32(s_col + col_slot<kTileN>(1, half * kColsPerHalf));
   const uint32_t out_addr = out.buf != nullptr ? smem_u32(out.buf) : 0u;
 
   float s1 = 0.f, s2 = 0.f, shift = 0.f;     // statistics of (y - shift), shift = the block's first value: sums stay small
@@ -287,7 +316,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
 #pragma unroll
   for (int chunk = 0; chunk < kChunks; ++chunk) {
     acc_chunk(acc, chunk, scratch, r);
-    const int col0 = col_tile0 + half * kColsPerWarp + chunk * 32;
+    const int col0 = col_tile0 + half * kColsPerHalf + chunk * 32;
     // dual output: every 64-column slab exists twice — pre-activation (even slab number, buffer 0) and activation (odd, buffer 1)
     const bool dual = !kTower && ep.dual != 0 && out.buf != nullptr;
     const uint32_t slab_pre = out.slab_seq + 2u * static_cast<uint32_t>(chunk / kChunksPerSlab);
@@ -299,10 +328,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
       mbar_wait(&out.empty_bar[slab_buf], ((slab_q >> 1) & 1u) ^ 1u);
     }
     if (col0 < N) {        // N is a multiple of 32 (checked on the host) -> whole chunk in or out
-      // kSubPairs packed pairs (2 columns each) go through every step together: each run-time option is ONE warp-uniform branch
-      // around a basic block of kSubPairs independent dependency chains for the scheduler to interleave (more chains, more registers).
-      constexpr int kSubPairs = 8;
-      const int rloc = epi_row(quarter, lane_id());
 #pragma unroll
       for (int sub = 0; sub < 16 / kSubPairs; ++sub) {
         const int lc = chunk * 32 + sub * kSubPairs * 2;             // first column of this sub-block inside the warp's slice
@@ -423,22 +448,23 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
     if (chunk == kChunks - 1 && !kTower && ep.stats_out != nullptr && row_ok) {
       // statistics are final once the last chunk's values exist; written BEFORE the last slab is handed over so that the store
       // warp's tile-done release (dependent GEMMs of the same launch read them) covers these stores too
-      const int slot = (col_tile0 + half * kColsPerWarp) / kColsPerWarp;
+      const int slot = (col_tile0 + half * kColsPerHalf) / kColsPerHalf;
       long long srow = row;
       if (!kTower && ep.wm_s != 0) srow = window_major_row(row, ep.wm_s);
       if (slot < ep.stats_out_slots) {
         // (mean, M2) of this 128-column block: mean = shift + s1/n, M2 = s2 - s1^2/n  (deviations from `shift` are O(std): no cancellation)
-        constexpr float inv_n = 1.0f / kColsPerWarp;
+        constexpr float inv_n = 1.0f / kColsPerHalf;
         const float dm = __fmul_rn(s1, inv_n);
         reinterpret_cast<float2*>(ep.stats_out)[srow * ep.stats_out_slots + slot] =
             make_float2(__fadd_rn(shift, dm), fmaxf(fmaf(-s1, dm, s2), 0.f));
       }
     }
     if (out.buf != nullptr && (chunk % kChunksPerSlab) == kChunksPerSlab - 1) {
-      // slab complete: make the generic-proxy writes visible to the async proxy, then one arrive per warp hands it to the store warp
+      // slab complete: make the generic-proxy writes visible to the async proxy, then one arrive per warp and column half hands
+      // it to the store warp
       fence_proxy_async_smem();
       __syncwarp();
-      if (lane_id() == 0) {
+      if ((lane_id() & 15u) == 0) {
         if (dual) mbar_arrive(&out.full_bar[slab_pre & 1u]);
         mbar_arrive(&out.full_bar[slab_buf]);
       }
@@ -455,8 +481,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
 //     phase V: v' = y_v . (gamma_v W_iv)^T                     -> epilogue: folded LayerNorm, p * v', halving exchange over the window's
 //              lanes, store the window's 128 context channels of the head
 //   Both phases use the same accumulator registers one after the other; the producer keeps the ring full in the meantime.
-//   Thread == key row; column half (warps 0-3 / 4-7) == head of the pair.  k' and v' never exist in memory (fp32, unrounded, in
-//   registers): the [R,1024] x 2 round trip through HBM and the separate attention kernel are gone.
+//   Thread == key row; column half (lanes 0-15 / 16-31 of every epilogue warp) == head of the pair.  k' and v' never exist in
+//   memory (fp32, unrounded, in registers): the [R,1024] x 2 round trip through HBM and the separate attention kernel are gone.
 // ------------------------------------------------------------------------------------------------
 struct AttnParams {
   const __nv_bfloat16* qp;      // [Q, 1024] q', row = window index (= query index), scaled
@@ -484,7 +510,7 @@ __device__ __forceinline__ float bf16x2_get(const uint4& v, int i) {      // i i
   return (i & 1) ? bf16_hi(w) : bf16_lo(w);
 }
 
-// Phase K epilogue: returns this row's softmax weight p for head `head`.  s_vec: [wsum | cst][256] of the tile's two heads.
+// Phase K epilogue: returns this row's softmax weight p for head `head`.  s_vec: wsum | cst of the tile's two heads (col_slot).
 __device__ __forceinline__ float attn_scores(const AttnParams& at, int M, const float (&acc)[2][64], uint32_t scratch, int row, int head,
                                              int half, const float* s_vec) {
   const int W = at.s * at.s;
@@ -492,8 +518,8 @@ __device__ __forceinline__ float attn_scores(const AttnParams& at, int M, const 
   float mu = 0.f, rstd = 0.f;
   if (row_ok) ln_row_stats(at.stats_k, row, at.stats_slots, at.ln_inv_dim, at.ln_eps, mu, rstd);
   const long long window = row / W;
-  const float* wsum = s_vec + half * 128;
-  const float* cst = s_vec + 256 + half * 128;
+  const float* wsum = s_vec + col_slot<256>(0, half * 128);
+  const float* cst = s_vec + col_slot<256>(1, half * 128);
   const uint4* qrow = reinterpret_cast<const uint4*>(at.qp + window * 1024 + head * 128);
   uint32_t r[32];
   float score = 0.f;
@@ -528,8 +554,8 @@ __device__ __forceinline__ void attn_pv(const AttnParams& at, int M, const float
   float mu = 0.f, rstd = 0.f;
   if (row_ok) ln_row_stats(at.stats_v, row, at.stats_slots, at.ln_inv_dim, at.ln_eps, mu, rstd);
   const long long window = row / W;
-  const float* wsum = s_vec + half * 128;
-  const float* cst = s_vec + 256 + half * 128;
+  const float* wsum = s_vec + col_slot<256>(0, half * 128);
+  const float* cst = s_vec + col_slot<256>(1, half * 128);
   uint32_t r[32];
 #pragma unroll
   for (int chunk = 0; chunk < 4; ++chunk) {
@@ -573,8 +599,8 @@ __device__ __forceinline__ void stage_col_vectors(const GemmEpilogue& ep, int N,
   for (int c = epi_tid; c < kTileN; c += kEpiThreads) {
     const int col = col_tile0 + c;
     const bool ok = col < N;
-    s_col[c] = (ok && ep.col_a != nullptr) ? __ldg(ep.col_a + col) : 0.f;
-    s_col[kTileN + c] = (ok && ep.col_b != nullptr) ? __ldg(ep.col_b + col) : 0.f;
+    s_col[col_slot<kTileN>(0, c)] = (ok && ep.col_a != nullptr) ? __ldg(ep.col_a + col) : 0.f;
+    s_col[col_slot<kTileN>(1, c)] = (ok && ep.col_b != nullptr) ? __ldg(ep.col_b + col) : 0.f;
   }
   named_bar_sync(kEpiBarrierId, kEpiThreads);
 }
@@ -588,7 +614,7 @@ struct GemmConfig {
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = kBlockN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kColStageBytes = 2 * kBlockN * 4;   // [col_a | col_b][kBlockN] floats
+  static constexpr int kColStageBytes = col_slot<kBlockN>(2, 0) * 4;   // [col_a | col_b], col_slot layout
   static constexpr int kBarrierBytes = 2 * kStages * 8;
   static constexpr int kSmemBytes = kStages * kStageBytes + kScratchBytes + kColStageBytes + kBarrierBytes + 1024;  // +1024: manual alignment
   static_assert(kSmemBytes <= 232448, "shared memory budget of an sm_90 SM (227 KiB)");
@@ -600,7 +626,6 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
                int a_seg_rows, GemmEpilogue ep) {
   using Cfg = GemmConfig<kBlockN>;
   constexpr int kStages = Cfg::kStages;
-  constexpr int kN = kBlockN / 2;                  // columns per warpgroup
   static_assert(kBlockN == 128 || kBlockN == 256, "BLOCK_N");
   static_assert(kTower || !kF16, "f16 instantiations are the tower's");
 
@@ -667,10 +692,11 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     // ======================================= MMA + epilogue (warpgroup = column half) =============
     setmaxnreg_inc<kMmaRegs>();
     const int e = warp_idx - kEpiWarp0;
-    const int quarter = warp_idx & 3;
     const int half = e >> 2;
+    const int rloc = epi_row_1cta(warp_idx & 3, lane);
     const int epi_tid = e * 32 + static_cast<int>(lane);
     const uint32_t scratch = smem_u32(s_scratch + e * kScratchBytesPerWarp);
+    constexpr int kN = kBlockN / 2;                  // columns per warpgroup
     int stage = 0;
     uint32_t phase = 0;
     float acc[2][kN / 2];
@@ -678,11 +704,11 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       const int m_blk = tile / num_n_blocks;
       const int n_blk = tile - m_blk * num_n_blocks;
       stage_col_vectors<kBlockN>(ep, N, n_blk * kBlockN, s_col, epi_tid, true);
-      mma_tile<kN, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, half * kN * kBlockK * 2, full_bar, empty_bar, kStages, stage, phase,
-                               num_k_blocks);
+      mma_tile<kN, 2, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, 0, Cfg::kABytes + half * kN * kBlockK * 2, full_bar, empty_bar, kStages, stage,
+                                  phase, num_k_blocks);
       const OutStage no_stage{nullptr, nullptr, nullptr, 0u};
-      epilogue_tile<kBlockN, kTower, kF16>(ep, M, N, acc, scratch, m_blk * kBlockM + epi_row(quarter, lane), n_blk * kBlockN, quarter, half, s_col,
-                                     no_stage);
+      epilogue_tile<kBlockN, kTower, kF16>(ep, M, N, acc, scratch, m_blk * kBlockM + rloc, rloc, n_blk * kBlockN, half, s_col,
+                                           no_stage);
     }
   }
 }
@@ -702,7 +728,7 @@ struct Gemm2Config {
   static constexpr int kBBytes = kTileN * kBlockK * 2;           // the whole B tile
   static constexpr int kStageBytes = kABytes + kBBytes;          // 48 KiB
   static constexpr int kOutBytes = 2 * kOutBufs * kOutSlabBytes; // [2 column halves][kOutBufs] output slabs for TMA stores
-  static constexpr int kColStageBytes = 2 * kTileN * 4;          // [col_a | col_b][kTileN] floats, ONE buffer (barrier before it is rewritten)
+  static constexpr int kColStageBytes = col_slot<kTileN>(2, 0) * 4;   // [col_a | col_b], col_slot layout, ONE buffer (barrier before it is rewritten)
   static constexpr int kBarrierBytes = (2 * kStages + 4 * kOutBufs) * 8;   // ring + slab full/empty per half
   // 3 stages x 48 KiB + 4 x 16 KiB slabs + 16 KiB transpose scratch + 2 KiB + barriers = 226.1 KiB of the 227 KiB an SM offers: the
   // dynamic shared memory is declared 1024-byte aligned (no alignment slack), and the per-column vectors are single-buffered
@@ -822,7 +848,6 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
   using Cfg = Gemm2Config;
   constexpr int kStages = Cfg::kStages;
   constexpr int kTileN = Cfg::kTileN;
-  constexpr int kN = kTileN / 2;                                // columns per warpgroup
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];     // 1 KiB aligned: swizzle atoms of the operand tiles and output slabs
   uint8_t* smem = smem_raw;
@@ -857,7 +882,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       mbar_init(&empty_bar[i], kNumEpiWarps);            // one arrive per MMA warp
     }
     for (int i = 0; i < 2 * Cfg::kOutBufs; ++i) {
-      mbar_init(&slab_full_bar[i], kNumEpiWarps / 2);    // one arrive per epilogue warp of the column half
+      mbar_init(&slab_full_bar[i], kNumEpiWarps);        // one arrive per epilogue warp (from its 16 lanes of the column half)
       mbar_init(&slab_empty_bar[i], 1);                  // the half's store warp
     }
     fence_barrier_init();
@@ -869,17 +894,17 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
   grid_launch_dependents();                // the next kernel's CTAs may take over SMs as ours exit (they block in their own wait)
   if (warp_idx < kNumEpiWarps) {
     setmaxnreg_inc<kMmaRegs>();
-    // ======================================= MMA + epilogue (own 128 rows, warpgroup = column half) ==
+    // ======================================= MMA + epilogue (own 128 rows, warpgroup = 64-row block) =
     const int e = warp_idx - kEpiWarp0;
-    const int quarter = warp_idx & 3;
-    const int half = e >> 2;
+    const int wg = e >> 2;
+    const int rloc = epi_row(wg, warp_idx & 3, lane);
+    const int half = epi_half(lane);
     const int epi_tid = e * 32 + static_cast<int>(lane);
     const uint32_t scratch = smem_u32(s_scratch + e * kScratchBytesPerWarp);
-    const int b_off = half * kN * kBlockK * 2;                  // this warpgroup's columns of the stage's B tile
     int stage = 0;
     uint32_t phase = 0;
     uint32_t slab_seq = 0;
-    float acc[2][kN / 2];
+    float acc[2][kTileN / 4];
     if (!kTower && grp.front.x0 != nullptr) {
       // point queries: this CTA's share of the (query, 8-channel vector) items, 128 vectors per query
       const FrontWork& fw = grp.front;
@@ -920,7 +945,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       const GemmProblem& pr = *t.pr;
       float* s_col = s_col_base;
       const int row_tile0 = t.m_blk * Cfg::kTileM + static_cast<int>(cta_rank) * kBlockM;
-      const int row = row_tile0 + epi_row(quarter, lane);
+      const int row = row_tile0 + rloc;
       if (!kTower && pr.kind == 1) {
         const AttnParams& at = pr.attn;
         const int head = t.n_blk * 2 + half;                 // column half == head of the tile's pair
@@ -928,12 +953,12 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
         vec.col_a = at.wsum_k;
         vec.col_b = at.cst_k;
         stage_col_vectors<kTileN>(vec, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
-        mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
+        mma_tile<kTileN, 1, 0, 0>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
         const float p = attn_scores(at, pr.M, acc, scratch, row, head, half, s_col);
         vec.col_a = at.wsum_v;
         vec.col_b = at.cst_v;
         stage_col_vectors<kTileN>(vec, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
-        mma_tile<kN, 0, 0>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
+        mma_tile<kTileN, 1, 0, 0>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
         attn_pv(at, pr.M, acc, scratch, row, head, half, p, s_col);
         if (at.done_counter != nullptr) {
           named_bar_sync(kEpiBarrierId, kEpiThreads);       // every epilogue thread's ctx stores are issued ...
@@ -947,15 +972,15 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       stage_col_vectors<kTileN>(pr.ep, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
       const int n_kb = t.kb1 - t.kb0;
       if (!kTower && pr.ab_mn_major == 1)
-        mma_tile<kN, 1, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
+        mma_tile<kTileN, 1, 1, 1>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, n_kb);
       else if (!kTower && pr.ab_mn_major == 2)
-        mma_tile<kN, 0, 1>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
+        mma_tile<kTileN, 1, 0, 1>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, n_kb);
       else
-        mma_tile<kN, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, Cfg::kABytes, b_off, full_bar, empty_bar, kStages, stage, phase, n_kb);
+        mma_tile<kTileN, 1, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, n_kb);
       const OutStage out{pr.use_tma_store ? s_out + half * Cfg::kOutBufs * kOutSlabBytes : nullptr, slab_full_bar + half * Cfg::kOutBufs,
                          slab_empty_bar + half * Cfg::kOutBufs, slab_seq};
       if (pr.use_tma_store) slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);     // slabs per tile and column half
-      epilogue_tile<kTileN, kTower, kF16>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, quarter, half, s_col, out,
+      epilogue_tile<kTileN, kTower, kF16, 4>(pr.ep, pr.M, pr.N, acc, scratch, row, rloc, t.n_blk * kTileN, half, s_col, out,
                                     static_cast<long long>(t.split) * pr.c_split_stride);
     }
   } else {
@@ -1081,7 +1106,7 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
     }
   } else if (warp_idx == kStoreWarp0 || warp_idx == kStoreWarp0 + 1) {
     // ======================================= store warps (both CTAs, one per column half) =========
-    // Walks the same tile sequence as the epilogue warps of its half.  Per slab: wait until the 4 epilogue warps have written
+    // Walks the same tile sequence as the epilogue warps.  Per slab: wait until the 8 epilogue warps have written their rows of
     // it (mbarrier), issue the TMA store(s) — plain 2-D box, clipped 3-D boxes for segmented rows, one per peer GPU for the
     // fused all-gather —, wait until the copy engine has READ the buffer and hand it back.  Per tile of a GEMM that others in
     // this launch depend on: wait for the stores to be PERFORMED, then publish the tile (release) on its row block's counter.
