@@ -141,7 +141,9 @@ for fn in ("tp_backward", "tp_backward_inputs"):
         (fn, dict(ws=None), BAD), (fn, dict(n=0), BAD), (fn, dict(n=0, s=5), BAD), (fn, dict(h=100), BAD), (fn, dict(h=100, s=5), BAD),
         (fn, dict(xms=XMS + 8), BAD), (fn, dict(xms=XMS - 4096), BAD),      # the backward takes a contiguous stack
         (fn, dict(w=NULL_W), BAD), (fn, dict(g=NULL_G), BAD),
+        (fn, dict(n=MAX_ROWS), BAD), (fn, dict(n=MAX_ROWS, s=5), BAD),      # the forwards' row limit holds for the backward too
     ]
+CASES += [("tp_backward_layers", dict(n=MAX_ROWS), BAD)]
 CASES += [
     ("tp_backward_inputs", dict(packed=None), BAD),                          # d_xm reads [W_k0; W_v0] from the packed weights
     ("tp_backward_inputs", dict(dx0=P + 2), BAD), ("tp_backward_inputs", dict(dxm=P + 8), BAD),
@@ -165,3 +167,13 @@ def test_entry_point_status(case):
     for k, v in over.items():
         a[k] = C.byref(_weights(null_last=True)) if v in (NULL_W, NULL_G) else v
     assert _call(fn, a) == getattr(_lib(), "TP_ERR_" + want)
+
+
+@pytest.mark.parametrize("query", ["tp_workspace_bytes", "tp_train_saved_bytes", "tp_backward_workspace_bytes"])
+def test_size_queries_stop_at_the_row_limit(query):
+    """Every size query gives a size up to the largest batch the entry points take (MAX_ROWS - 1 crops) and 0 past it, like the
+    entry points' own refusal: no caller allocates a workspace for a batch nothing will run."""
+    fn = getattr(_lib().lib, query)
+    for s, h in ((1, 4096), (2, 4096), (3, 896), (24, 160)):
+        assert fn(MAX_ROWS - 1, s, h) > 0, (s, h)
+        assert fn(MAX_ROWS, s, h) == 0 and fn(1 << 40, s, h) == 0, (s, h)

@@ -847,6 +847,10 @@ WorkLayout work_layout(long long n_crops, int s, int H) {
 
 bool valid_hidden(int H) { return H >= 32 && H % 32 == 0 && H <= 65536; }
 
+// Most crops one projector call takes, forward or backward: 576 N token rows stay within the GEMMs' 32-bit row count (0x7fff0000).
+// The size queries return 0 past it.
+constexpr long long kMaxCrops = 0x7fff0000ll / kTokens;
+
 template <int S>
 int launch_front(const __nv_bfloat16* x0, long long x0_stride, __nv_bfloat16* q, long long Q, cudaStream_t stream) {
   const long long threads = Q * 128;
@@ -894,8 +898,10 @@ int launch_attn_s(int s, const __nv_bfloat16* qp, const __nv_bfloat16* kp, const
 }
 
 // out[c, r] = in[r, c]  (in: [rows, cols] bf16, row stride ld_in; out: [cols, rows], row stride ld_out)
+// Row tiles go on grid.x, column tiles on grid.y (at most 65535: cols <= 2,097,120; a projector's hidden size is at most 65536).
 int launch_transpose(const void* in, long long ld_in, void* out, long long ld_out, long long rows, int cols, cudaStream_t stream) {
-  const dim3 grid(static_cast<unsigned>((cols + 31) / 32), static_cast<unsigned>((rows + 31) / 32));
+  if ((rows + 31) / 32 > 0x7fffffffll || (cols + 31) / 32 > 65535) return TP_ERR_INVALID_ARGUMENT;
+  const dim3 grid(static_cast<unsigned>((rows + 31) / 32), static_cast<unsigned>((cols + 31) / 32));
   transpose_kernel<<<grid, dim3(32, 8), 0, stream>>>(static_cast<const __nv_bfloat16*>(in), ld_in, static_cast<__nv_bfloat16*>(out), ld_out, rows,
                                                       cols);
   TP_CUDA(cudaGetLastError()); ++g_launch_count;
@@ -999,7 +1005,7 @@ int tp_pack_weights(const tp_weights* w, int hidden, void* packed, size_t packed
 }
 
 size_t tp_workspace_bytes(int64_t n_crops, int scale_factor, int hidden) {
-  if (n_crops <= 0 || scale_factor <= 0 || kGrid % scale_factor != 0 || !valid_hidden(hidden)) return 0;
+  if (n_crops <= 0 || n_crops > kMaxCrops || scale_factor <= 0 || kGrid % scale_factor != 0 || !valid_hidden(hidden)) return 0;
   return work_layout(n_crops, scale_factor, hidden).total;
 }
 
@@ -1125,7 +1131,7 @@ int forward_impl(const void* packed, const Features& f, int64_t n_crops, int sca
                  int64_t out_crop_rows, void* const* peer_out, int n_peers, void* workspace, size_t workspace_bytes, void* stream_) {
   if (scale_factor <= 0 || kGrid % scale_factor != 0) return TP_ERR_BAD_SCALE_FACTOR;          // builder.py:51-52
   if (packed == nullptr || !f.valid() || out == nullptr || workspace == nullptr || n_crops <= 0 || !valid_hidden(hidden) ||
-      n_crops * kTokens > 0x7fff0000ll)
+      n_crops > kMaxCrops)
     return TP_ERR_INVALID_ARGUMENT;
   DeviceInfo dev;
   TP_TRY(device_info(&dev));
@@ -1148,9 +1154,12 @@ int forward_impl(const void* packed, const Features& f, int64_t n_crops, int sca
   bufs.stats_v = bufs.stats_k + 2 * kStatSlots * R;
   bufs.stats_q = bufs.stats_v + 2 * kStatSlots * R;     // every slot is written by the producing GEMM: no memset needed
 
-  // Launch plan.  Large batches: 4 launches — [S], chain A = {[1], [2], [3]} and chain B = {[4], [5]} as ONE persistent CTA-pair
-  // launch each (stages ordered by per-row-block tile counters instead of kernel boundaries), [A] in between.  Small batches
-  // (one-CTA tiles win): the same stages as separate launches.
+  // Launch plan.  s = 2 / 4 with hidden % 256 == 0: the fused plan below, one launch at every batch size.  Otherwise chain A =
+  // {[S], [1], [2], [3]} and chain B = {[4], [5]} would each run as ONE persistent CTA-pair launch (stages ordered by per-row-block
+  // tile counters) if choose_kernel, costing the chain's items as one launch, put every one of them on the pair kernel; on an H100
+  // (132 SMs) it never does at the default mode (some item of each chain goes to a one-CTA kernel at every N), so the stages run as
+  // separate launches, [A] in between: 7 to 11 launches depending on N (tests/test_projector_batches_gpu.py records the plans and
+  // which items block each chain).  TP_GEMM_MODE=2 takes the chains: 3 launches.
   //   [S] point queries            builder.py:117-118   (inside chain A: done by the epilogue warps before their first tile)
   //   [1] h_kv = GELU(xm [W_k0;W_v0]^T + b)                                 :112-113 first linears, xm read once
   //   [2] y_k | y_v | y_q   = second linears k/v + q_proj_1 (+ row statistics for the LayerNorms)   :112-113, :120

@@ -57,8 +57,8 @@ __device__ __forceinline__ float gelu_grad(float z) {
 __global__ void transpose_kernel(const __nv_bfloat16* __restrict__ in, long long ld_in, __nv_bfloat16* __restrict__ out, long long ld_out,
                                  long long rows, int cols) {
   __shared__ __nv_bfloat16 tile[32][34];
-  const long long r0 = static_cast<long long>(blockIdx.y) * 32;
-  const int c0 = blockIdx.x * 32;
+  const long long r0 = static_cast<long long>(blockIdx.x) * 32;     // row tiles on grid.x (up to 2^31 - 1 of them; grid.y stops at 65535)
+  const int c0 = blockIdx.y * 32;
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     const long long r = r0 + i;
     const int c = c0 + threadIdx.x;
