@@ -10,8 +10,10 @@ from .projector import TokenPackerB200, TokenPacker, build_vision_projector, Ide
 from .hd import Image_Patch, hd_grid, hd_tile, hd_tile_batch, hd_preprocess_batch, hd_plan, hd_assemble, hd_seq_len
 from .clip import clip_preprocess_batch
 from .jpeg import decode_jpeg_batch, jpeg_unsupported
+from .png import decode_png_batch, png_unsupported
 from .splice import splice_multimodal, splice_plan
 from .tower import CLIPVisionTowerB200
 
 __all__ = ["TokenPackerB200", "TokenPacker", "build_vision_projector", "IdentityMap", "Image_Patch", "hd_grid", "hd_tile", "hd_tile_batch",
-           "hd_preprocess_batch", "hd_plan", "hd_assemble", "hd_seq_len", "clip_preprocess_batch", "decode_jpeg_batch", "jpeg_unsupported", "splice_multimodal", "splice_plan", "CLIPVisionTowerB200"]
+           "hd_preprocess_batch", "hd_plan", "hd_assemble", "hd_seq_len", "clip_preprocess_batch", "decode_jpeg_batch", "jpeg_unsupported",
+           "decode_png_batch", "png_unsupported", "splice_multimodal", "splice_plan", "CLIPVisionTowerB200"]

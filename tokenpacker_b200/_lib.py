@@ -4,7 +4,7 @@ There is deliberately no fallback: if the shared library is missing the import f
 Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
 include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h, include/tokenpacker_b200_clip_tower.h,
 include/tokenpacker_b200_clip_tower_f16.h, include/tokenpacker_b200_clip_tower_train.h, include/tokenpacker_b200_clip_tower_ckpt.h,
-include/tokenpacker_b200_clip_tower_embed.h and include/tokenpacker_b200_jpeg.h one to one.
+include/tokenpacker_b200_clip_tower_embed.h, include/tokenpacker_b200_jpeg.h and include/tokenpacker_b200_png.h one to one.
 """
 from __future__ import annotations
 
@@ -273,6 +273,42 @@ JPEG_SIGNATURES = {
 }
 
 
+# the same for include/tokenpacker_b200_png.h (PNG files decoded on the GPU, byte for byte as PIL)
+class TpPngImage(C.Structure):
+    """tp_png_image: one row of the decode plan."""
+    _fields_ = [(n, C.c_int32) for n in ("reason", "h", "w", "depth", "color_type", "channels", "row_bytes", "filter_bpp",
+                                         "palette_entries", "window")] + \
+               [(n, C.c_int64) for n in ("palette_offset", "stream_offset", "stream_bytes", "raw_bytes", "block_capacity", "mask_offset",
+                                         "spec_offset", "block_offset", "raw_offset", "src_offset", "out_offset", "pixel0")]
+
+
+class TpPngBlock(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("start_bit", "end_bit", "out_offset", "out_bytes", "flags")]
+
+
+class TpPngTotals(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("staged_bytes", "output_bytes", "workspace_bytes", "max_raw_bytes", "pixels")]
+
+
+class TpPngStatus(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("status", "blocks", "serial_blocks", "candidates")]
+
+
+TP_PNG_SUPPORTED = 0
+TP_PNG_PALETTE_BYTES = 768
+TP_PNG_SPAN_BITS, TP_PNG_SLOTS, TP_PNG_MIN_BLOCK_BITS = 256, 4, 10
+(TP_PNG_STATUS_OK, TP_PNG_STATUS_BLOCK_TYPE, TP_PNG_STATUS_CODE_LENGTHS, TP_PNG_STATUS_SYMBOL, TP_PNG_STATUS_DISTANCE,
+ TP_PNG_STATUS_STORED, TP_PNG_STATUS_TRUNCATED, TP_PNG_STATUS_DATA_SIZE, TP_PNG_STATUS_ADLER, TP_PNG_STATUS_FILTER) = range(10)
+PNG_SIGNATURES = {
+    "tp_png_plan": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int64, C.POINTER(TpPngImage), C.c_void_p, C.c_void_p,
+                              C.POINTER(TpPngTotals)]),
+    "tp_png_workspace_bytes": (C.c_size_t, [C.POINTER(TpPngImage), C.c_int64]),
+    "tp_png_reason_string": (C.c_char_p, [C.c_int]),
+    "tp_png_decode_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t,
+                                      C.c_void_p, C.c_void_p]),
+}
+
+
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
@@ -282,7 +318,7 @@ def _load():
     for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
                                       **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES,
                                       **CLIP_TOWER_TRAIN_SIGNATURES, **CLIP_TOWER_CKPT_SIGNATURES,
-                                      **CLIP_TOWER_EMBED_SIGNATURES, **JPEG_SIGNATURES}.items():
+                                      **CLIP_TOWER_EMBED_SIGNATURES, **JPEG_SIGNATURES, **PNG_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

@@ -22,6 +22,7 @@
 #include "../../include/tokenpacker_b200_input_grad.h"
 #include "../../include/tokenpacker_b200_layers.h"
 #include "../../include/tokenpacker_b200_jpeg.h"
+#include "../../include/tokenpacker_b200_png.h"
 #include "tp_gemm.cuh"
 #include "tp_kernels.cuh"
 #include "tp_backward.cuh"
@@ -29,6 +30,7 @@
 #include "tp_clip_tower_train.cuh"
 #include "tp_clip_tower_embed.cuh"
 #include "tp_jpeg.cuh"
+#include "tp_png.cuh"
 
 namespace {
 
@@ -1922,3 +1924,4 @@ int tp_hd_fill_separators(void* out, int hidden, const int64_t* sep_rows, int64_
 #include "tp_clip_tower_ckpt.inl"
 #include "tp_clip_tower_embed.inl"
 #include "tp_jpeg.inl"
+#include "tp_png.inl"
