@@ -17,10 +17,12 @@
 // CTA = 384 threads, persistent over output tiles:
 //   warps 0-7   two MMA + epilogue warpgroups, one per 64-row block of the CTA's 128 rows: one wgmma m64nNk16 per k16 step over
 //               the whole N-column tile (N/2 fp32 accumulators per thread), so each warpgroup reads its A block once and the B tile
-//               once per k-step; then the epilogue on the same registers: each warp turns its fragments into thread == output row
-//               form (lanes 0-15: column half 0, lanes 16-31: column half 1 of the warp's 16 rows) through a 2 KiB shared-memory
-//               transpose (32 columns at a time), fused per-row / per-column math, swizzled shared-memory slabs (16-byte stores)
-//               or direct 16-byte global stores
+//               once per k-step; then the epilogue on the same registers.  Pair-kernel tiles stored through TMA (not the tower's):
+//               fused per-row / per-column math on the fragments in place, stmatrix into the swizzled shared-memory slabs
+//               (epilogue_tile_frag).  Everything else (KV-attention, direct global stores, the one-CTA kernel, the tower): each
+//               warp turns its fragments into thread == output row form (lanes 0-15: column half 0, lanes 16-31: column half 1 of
+//               the warp's 16 rows) through a 2 KiB shared-memory transpose (32 columns at a time), fused per-row / per-column
+//               math, swizzled shared-memory slabs (16-byte stores) or direct 16-byte global stores
 //   warps 8, 9  store warps of the pair kernel (one per column half): wait for a finished slab on an mbarrier, issue its TMA
 //               store(s), hand the buffer back, and — for GEMMs that other GEMMs of the same launch depend on — publish each
 //               finished tile to a global counter.  The epilogue warps never wait for a store.
@@ -605,6 +607,191 @@ __device__ __forceinline__ void stage_col_vectors(const GemmEpilogue& ep, int N,
   named_bar_sync(kEpiBarrierId, kEpiThreads);
 }
 
+// The pair kernel's form of the same: the copies are issued with cp.async (zero fill for columns >= N and null vectors) and land
+// while the tile's MMAs run; col_vectors_ready() before the epilogue reads them.  The caller has passed a barrier since the
+// previous tile's vectors were last read (the buffer is single).  16-byte pieces (col_slot keeps them 16-byte aligned in shared
+// memory) unless a vector's address is not 16-byte aligned; a null vector is zeroed with plain shared stores (no copy, no source
+// address), and a piece past N reads 0 bytes from the vector's first element.
+template <int kTileN>
+__device__ __forceinline__ void stage_col_vectors_async(const float* col_a, const float* col_b, int N, int col_tile0, float* s_col,
+                                                        int epi_tid) {
+#pragma unroll
+  for (int vec = 0; vec < 2; ++vec) {
+    const float* v = vec == 0 ? col_a : col_b;
+    if ((reinterpret_cast<uintptr_t>(v) & 15u) == 0) {
+      for (int c = 4 * epi_tid; c < kTileN; c += 4 * kEpiThreads) {      // N is a multiple of 32: a piece is all in or all out
+        const int col = col_tile0 + c;
+        const uint32_t dst = smem_u32(s_col + col_slot<kTileN>(vec, c));
+        if (v == nullptr) sts_u4(dst, 0u, 0u, 0u, 0u);               // made visible by col_vectors_ready's barrier
+        else cp_async_16(dst, col < N ? v + col : v, col < N ? 16u : 0u);
+      }
+    } else {
+      for (int c = epi_tid; c < kTileN; c += kEpiThreads) {
+        const int col = col_tile0 + c;
+        cp_async_4(smem_u32(s_col + col_slot<kTileN>(vec, c)), col < N ? v + col : v, col < N ? 4u : 0u);
+      }
+    }
+  }
+}
+__device__ __forceinline__ void col_vectors_ready() {
+  cp_async_wait_all();
+  named_bar_sync(kEpiBarrierId, kEpiThreads);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Pair kernel, tiles stored through the TMA slabs (not the tower's instantiations): the epilogue works on the wgmma m64n256
+// fragments where they are, with no transpose.  Lane (g = lane / 4, q = lane % 4) of a warp holds rows g and g + 8 of the warp's 16
+// rows, columns 8 j + 2 q, +1 of both column halves; every value goes through the same explicit fma / add / mul sequence as in
+// epilogue_tile, so the bits do not depend on which thread computes them.  The packed bf16 pairs are already in the m8n8 matrix
+// fragment form: stmatrix writes each 8 x 8 block's rows to their 128B-swizzled slab positions.  The warp writes both column halves,
+// slab by slab with the halves interleaved so that both store warps stay busy, and hands each half-slab over with one arrive.
+//   Row statistics keep epilogue_tile's order (sequential over the 128 rounded columns of a row and half): once both halves of a
+// slab are written, lane l re-reads row l % 16, column half l / 16 of it in column order — before the next slab is written, which
+// with dual output reuses the same activation buffer; the last slab of each half is handed over only once the statistics are
+// stored, so that the store warp's tile-done release covers them.
+//   acc: [column half][fragment registers]; rloc_w0 / row_w0: tile row / global row of the warp's first row; s_out: the [2 halves]
+// [kOutBufs] slabs; full_bar / empty_bar: [2 halves][kOutBufs]; slab_seq: running slab number (both halves share it).
+// ------------------------------------------------------------------------------------------------
+template <int kOutBufs>
+__device__ __forceinline__ void epilogue_tile_frag(const GemmEpilogue& ep, int M, const float (&acc)[2][64], int row_w0, int rloc_w0,
+                                                   int col_tile0, const float* s_col, uint8_t* s_out, uint64_t* full_bar,
+                                                   uint64_t* empty_bar, uint32_t slab_seq) {
+  static_assert(kOutBufs == 2, "slab numbering: buffer = seq % 2");
+  constexpr int kColsPerHalf = 128;
+  const uint32_t lane = lane_id();
+  const uint32_t g = lane >> 2, q = lane & 3u;
+  const bool ln_fold = ep.col_a != nullptr;
+  const bool dual = ep.dual != 0;
+  const bool scale = ep.alpha != 1.0f;
+  const bool do_stats = ep.stats_out != nullptr;
+  uint64_t rstd2[2], nmu2[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = row_w0 + static_cast<int>(g) + 8 * r;
+    float mu = 0.f, rstd = 1.f;
+    if (ln_fold && row < M) ln_row_stats(ep.stats_in, row, ep.stats_in_slots, ep.ln_inv_dim, ep.ln_eps, mu, rstd);
+    rstd2[r] = pk2(rstd);
+    nmu2[r] = pk2(-mu);
+  }
+  const uint64_t alpha2 = pk2(ep.alpha);
+  // this lane's stmatrix row address: matrix m = lane / 8 of an x4 is (8-column group m / 2, rows 8 (m % 2) ..); rloc_w0 is a
+  // multiple of 16, so the row's swizzle (row & 7) is lane & 7
+  const uint32_t m_row = static_cast<uint32_t>(rloc_w0) + 8u * ((lane >> 3) & 1u) + (lane & 7u);
+  const uint32_t m_grp = lane >> 4;
+  const uint32_t out_addr = smem_u32(s_out);
+  const uint32_t sa_addr = smem_u32(s_col + col_slot<256>(0, 0)), sb_addr = smem_u32(s_col + col_slot<256>(1, 0));
+  // row statistics: this lane's row and column half, and its running sums of (y - shift), shift = the block's first value
+  const int st_r = static_cast<int>(lane & 15u), st_h = static_cast<int>(lane >> 4);
+  const uint32_t st_addr = out_addr + static_cast<uint32_t>(st_h * kOutBufs * kOutSlabBytes + (rloc_w0 + st_r) * kSlabRowBytes);
+  float s1 = 0.f, s2 = 0.f, shift = 0.f;
+#pragma unroll
+  for (int s = 0; s < kColsPerHalf / kSlabCols; ++s) {
+    // dual output: every 64-column slab exists twice — pre-activation (even slab number, buffer 0) and activation (odd, buffer 1)
+    const uint32_t slab_pre = slab_seq + 2u * static_cast<uint32_t>(s);
+    const uint32_t slab_q = dual ? slab_pre + 1u : slab_seq + static_cast<uint32_t>(s);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint64_t* full = full_bar + h * kOutBufs;
+      uint64_t* empty = empty_bar + h * kOutBufs;
+      // the TMA store that last used this staging buffer must have finished READING it (signalled by the store warp)
+      if (dual) mbar_wait(&empty[slab_pre & 1u], ((slab_pre >> 1) & 1u) ^ 1u);
+      mbar_wait(&empty[slab_q & 1u], ((slab_q >> 1) & 1u) ^ 1u);
+      const uint32_t half_addr = out_addr + static_cast<uint32_t>(h * kOutBufs * kOutSlabBytes) + m_row * kSlabRowBytes;
+#pragma unroll
+      for (int x = 0; x < kSlabCols / 16; ++x) {
+        // 8-column groups j0 = 8 s + 2 x and j0 + 1 of the half: v[2 jj + r] = row g + 8 r, columns 8 (j0 + jj) + 2 q, +1
+        uint64_t v[4];
+#pragma unroll
+        for (int jj = 0; jj < 2; ++jj) {
+          const int j = 8 * s + 2 * x + jj;
+          const uint32_t c = static_cast<uint32_t>(h * kColsPerHalf + 8 * j + (h ? kColPad : 0)) + 2u * q;    // col_slot offset
+          const uint64_t b2 = lds_f2(sb_addr + c * 4u);
+          if (ln_fold) {     // v = fma(rstd, fma(-mu, col_a, v), col_b): explicit fmas, the same in every instantiation
+            const uint64_t a2 = lds_f2(sa_addr + c * 4u);
+#pragma unroll
+            for (int r = 0; r < 2; ++r)
+              v[2 * jj + r] = fma2(rstd2[r], fma2(nmu2[r], a2, pk2(acc[h][4 * j + 2 * r], acc[h][4 * j + 2 * r + 1])), b2);
+          } else {
+#pragma unroll
+            for (int r = 0; r < 2; ++r) v[2 * jj + r] = add2(pk2(acc[h][4 * j + 2 * r], acc[h][4 * j + 2 * r + 1]), b2);
+          }
+        }
+        // 16-byte piece of the slab row: groups 2 x + m_grp, XOR-swizzled like TMA's SWIZZLE_128B
+        const uint32_t piece = ((2u * static_cast<uint32_t>(x) + m_grp) ^ (lane & 7u)) << 4;
+        uint32_t w[4];
+        if (dual) {        // the pre-activation slab
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            float lo, hi;
+            upk2(v[k], lo, hi);
+            w[k] = pack_bf16x2(lo, hi);
+          }
+          stmatrix_x4(half_addr + (slab_pre & 1u) * kOutSlabBytes + piece, w[0], w[1], w[2], w[3]);
+        }
+        if (ep.gelu) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) v[k] = gelu_erf_pk(v[k]);
+        }
+        if (scale) {       // alpha == 1 (every GEMM but in_proj_q): x * 1 is x, skip the multiply
+#pragma unroll
+          for (int k = 0; k < 4; ++k) v[k] = mul2(v[k], alpha2);
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          float lo, hi;
+          upk2(v[k], lo, hi);
+          w[k] = pack_bf16x2(lo, hi);
+        }
+        stmatrix_x4(half_addr + (slab_q & 1u) * kOutSlabBytes + piece, w[0], w[1], w[2], w[3]);
+      }
+      // slab written: make the generic-proxy writes visible to the async proxy, then one arrive per warp hands it to the store warp
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0 && !(do_stats && s == kColsPerHalf / kSlabCols - 1)) {
+        if (dual) mbar_arrive(&full[slab_pre & 1u]);
+        mbar_arrive(&full[slab_q & 1u]);
+      }
+    }
+    if (do_stats) {
+      // LayerNorm statistics of the ROUNDED values the next GEMM will read, from the warp's own rows of this slab (ordered by the
+      // __syncwarp above; only this warp writes them, and only after this read), in column order (deterministic)
+#pragma unroll
+      for (int ci = 0; ci < kSlabRowBytes / 16; ++ci) {
+        const uint4 u = lds_u4_ordered(st_addr + (slab_q & 1u) * kOutSlabBytes + static_cast<uint32_t>((ci ^ (st_r & 7)) << 4));
+        const uint32_t pk[4] = {u.x, u.y, u.z, u.w};
+        if (s == 0 && ci == 0) shift = bf16_lo(pk[0]);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float y0 = __fsub_rn(bf16_lo(pk[j]), shift), y1 = __fsub_rn(bf16_hi(pk[j]), shift);
+          s1 = __fadd_rn(s1, __fadd_rn(y0, y1));
+          s2 = fmaf(y0, y0, fmaf(y1, y1, s2));
+        }
+      }
+    }
+  }
+  if (do_stats) {
+    const int row = row_w0 + st_r;
+    const int slot = (col_tile0 + st_h * kColsPerHalf) / kColsPerHalf;
+    if (row < M && slot < ep.stats_out_slots) {
+      const long long srow = ep.wm_s != 0 ? window_major_row(row, ep.wm_s) : row;
+      // (mean, M2) of this 128-column block: mean = shift + s1/n, M2 = s2 - s1^2/n  (deviations from `shift` are O(std): no cancellation)
+      constexpr float inv_n = 1.0f / kColsPerHalf;
+      const float dm = __fmul_rn(s1, inv_n);
+      reinterpret_cast<float2*>(ep.stats_out)[srow * ep.stats_out_slots + slot] = make_float2(__fadd_rn(shift, dm), fmaxf(fmaf(-s1, dm, s2), 0.f));
+    }
+    __syncwarp();                              // every lane's statistics are stored before the last slabs are handed over
+    if (lane == 0) {
+      const uint32_t slab_pre = slab_seq + 2u * static_cast<uint32_t>(kColsPerHalf / kSlabCols - 1);
+      const uint32_t slab_q = dual ? slab_pre + 1u : slab_seq + static_cast<uint32_t>(kColsPerHalf / kSlabCols - 1);
+#pragma unroll
+      for (int h2 = 0; h2 < 2; ++h2) {
+        if (dual) mbar_arrive(&full_bar[h2 * kOutBufs + (slab_pre & 1u)]);
+        mbar_arrive(&full_bar[h2 * kOutBufs + (slab_q & 1u)]);
+      }
+    }
+  }
+}
+
 // ================================================================================================
 // One-CTA kernel: 128 x kBlockN tiles
 // ================================================================================================
@@ -949,16 +1136,15 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       if (!kTower && pr.kind == 1) {
         const AttnParams& at = pr.attn;
         const int head = t.n_blk * 2 + half;                 // column half == head of the tile's pair
-        GemmEpilogue vec;                                    // only col_a / col_b are read by the staging helper
-        vec.col_a = at.wsum_k;
-        vec.col_b = at.cst_k;
-        stage_col_vectors<kTileN>(vec, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
+        named_bar_sync(kEpiBarrierId, kEpiThreads);          // everyone is done reading the previous tile's vectors
+        stage_col_vectors_async<kTileN>(at.wsum_k, at.cst_k, pr.N, t.n_blk * kTileN, s_col, epi_tid);
         mma_tile<kTileN, 1, 0, 0>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
+        col_vectors_ready();
         const float p = attn_scores(at, pr.M, acc, scratch, row, head, half, s_col);
-        vec.col_a = at.wsum_v;
-        vec.col_b = at.cst_v;
-        stage_col_vectors<kTileN>(vec, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
+        named_bar_sync(kEpiBarrierId, kEpiThreads);          // everyone is done reading phase K's vectors
+        stage_col_vectors_async<kTileN>(at.wsum_v, at.cst_v, pr.N, t.n_blk * kTileN, s_col, epi_tid);
         mma_tile<kTileN, 1, 0, 0>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
+        col_vectors_ready();
         attn_pv(at, pr.M, acc, scratch, row, head, half, p, s_col);
         if (at.done_counter != nullptr) {
           named_bar_sync(kEpiBarrierId, kEpiThreads);       // every epilogue thread's ctx stores are issued ...
@@ -969,7 +1155,8 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
         }
         continue;
       }
-      stage_col_vectors<kTileN>(pr.ep, pr.N, t.n_blk * kTileN, s_col, epi_tid, true);
+      named_bar_sync(kEpiBarrierId, kEpiThreads);            // everyone is done reading the previous tile's vectors
+      stage_col_vectors_async<kTileN>(pr.ep.col_a, pr.ep.col_b, pr.N, t.n_blk * kTileN, s_col, epi_tid);
       const int n_kb = t.kb1 - t.kb0;
       if (!kTower && pr.ab_mn_major == 1)
         mma_tile<kTileN, 1, 1, 1>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, n_kb);
@@ -977,6 +1164,14 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
         mma_tile<kTileN, 1, 0, 1>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, n_kb);
       else
         mma_tile<kTileN, 1, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, n_kb);
+      col_vectors_ready();
+      if (!kTower && pr.use_tma_store) {
+        const int rloc_w0 = 64 * wg + 16 * (warp_idx & 3);
+        epilogue_tile_frag<Cfg::kOutBufs>(pr.ep, pr.M, acc, row_tile0 + rloc_w0, rloc_w0, t.n_blk * kTileN, s_col, s_out, slab_full_bar,
+                                          slab_empty_bar, slab_seq);
+        slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);                        // slabs per tile and column half
+        continue;
+      }
       const OutStage out{pr.use_tma_store ? s_out + half * Cfg::kOutBufs * kOutSlabBytes : nullptr, slab_full_bar + half * Cfg::kOutBufs,
                          slab_empty_bar + half * Cfg::kOutBufs, slab_seq};
       if (pr.use_tma_store) slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);     // slabs per tile and column half
