@@ -6,17 +6,19 @@
 
 extern "C" {
 
-// C[M, N] = epilogue(A[M, K] . B[N, K]^T) with the tower's epilogue: bias (fp32, may be NULL), residual R [M, ldr] (NULL: none),
-// gelu 0 / 2 (quick_gelu).  mode: 0 = the engine's own choice, 1 = one-CTA 128 x 256 tiles, 2 = the pair kernel.
-TP_API int tpc_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, void* c, int64_t ldc, int64_t m, int64_t n, int64_t k,
-                    const float* bias, const void* resid, int64_t ldr, int gelu, int mode, void* stream_) {
+// C[M, N] = epilogue(A[M, K] . B[N, K]^T) with the tower's epilogue: bias (fp32, may be NULL), residual R [M, ldr] (NULL: none; bf16,
+// or fp32 with resid_f32: the tower's mid-layer residual x'), gelu 0 / 2 (quick_gelu).  mode: 0 = the engine's own choice, 1 = one-CTA
+// 128 x 256 tiles, 2 = the pair kernel.
+TP_API int tpc_gemm_resid(const void* a, int64_t lda, const void* b, int64_t ldb, void* c, int64_t ldc, int64_t m, int64_t n, int64_t k,
+                          const float* bias, const void* resid, int64_t ldr, int resid_f32, int gelu, int mode, void* stream_) {
   if (a == nullptr || b == nullptr || c == nullptr || mode < 0 || mode > 2) return TP_ERR_INVALID_ARGUMENT;
   DeviceInfo dev;
   TP_TRY(device_info(&dev));
   GemmItem it{AOperand{a, lda, 0, 0}, b, ldb, m, n, k, clip_epilogue(c, ldc)};
   it.ep.col_b = bias;
-  it.ep.resid = static_cast<const __nv_bfloat16*>(resid);
+  it.ep.resid = resid;
   it.ep.ldr = ldr;
+  it.ep.resid_f32 = resid_f32;
   it.ep.gelu = gelu;
   TP_TRY(check_item(it));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -26,6 +28,12 @@ TP_API int tpc_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, void
   CUtensorMap ma, mb;
   TP_TRY(make_one_cta_maps(it, 256, &ma, &mb));
   return launch_gemm_t<256>(it, ma, mb, dev.sms, stream);
+}
+
+// tpc_gemm_resid with a bf16 residual
+TP_API int tpc_gemm(const void* a, int64_t lda, const void* b, int64_t ldb, void* c, int64_t ldc, int64_t m, int64_t n, int64_t k,
+                    const float* bias, const void* resid, int64_t ldr, int gelu, int mode, void* stream) {
+  return tpc_gemm_resid(a, lda, b, ldb, c, ldc, m, n, k, bias, resid, ldr, 0, gelu, mode, stream);
 }
 
 // ctx [n * 577, 1024] = attention of qkv [n * 577, 3072] (q pre-scaled), the kernel tp_clip_tower_forward runs in every layer

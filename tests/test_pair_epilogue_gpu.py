@@ -1,18 +1,26 @@
 """The pair kernel's fragment-direct epilogue (tiles stored through the TMA slabs: every value computed where the wgmma fragment holds
-it, bf16 written to the slabs with stmatrix, row statistics re-read from the slabs) against the one-CTA kernel, whose epilogue still
+it, 16-bit values written to the slabs with stmatrix, row statistics re-read from the slabs) against the one-CTA kernel, whose epilogue
 turns the fragments into one-row-per-thread form through shared memory: for every epilogue kind both store the same bits.
 
 Items and their NaN-sentinel output frames are those of tests/test_gemm_engine_gpu.py.  The pair kernel takes plain-form items
 only at N % 256 == 0 (narrower N runs on the one-CTA kernels alone), so N sweeps 256, 512 and 1024; M sweeps a single row, ragged
 row tiles and 36864 + 64 rows (the benchmarked batch's token count and a partial last row tile).  Window-major row statistics exist
 only inside the fused forward and are checked by tests/test_forward_stages_gpu.py.
+
+The CLIP tower's instantiations (bias, bf16 / f16 / fp32 residual, quick_gelu, alpha, f16 output, the patch GEMM's segmented store) go
+through the same comparison with the tower's own test hooks (tpc_gemm_resid, tpc_gemm_f16), from one row to the 64-crop batch's token
+count plus a partial row tile, at the tower's widths N = 1024 and 4096.
 """
+import ctypes as C
+
 import pytest
 import torch
 
+from test_clip_tower_forward_stages_gpu import F16, _lib, _ptr, i32, i64, p
 from test_gemm_engine_gpu import BF, GUARD, ONE_256, PAIR, Item, _bits, _run, _same_bits, hk  # noqa: F401  (hk: fixture)
 
 pytestmark = pytest.mark.gpu
+DEV = "cuda:0"
 
 KINDS = {
     "bias": dict(bias=True),
@@ -91,3 +99,73 @@ def test_pair_unaligned_column_vectors(hk, kind):
     _run(hk, [it], mode="2", expect=PAIR)
     it.check_guards()
     assert _same_bits(it.snapshot(), one)
+
+
+TOWER_KINDS = {
+    "bf16_bias_resid": dict(dtype=BF, bias=True, resid="x"),
+    "bf16_bias_resid_f32": dict(dtype=BF, bias=True, resid="f32"),
+    "bf16_quick_gelu": dict(dtype=BF, bias=True, gelu=2),
+    "bf16_quick_gelu_no_bias": dict(dtype=BF, gelu=2),
+    "f16_bias_resid": dict(dtype=F16, bias=True, resid="x"),
+    "f16_bias_resid_f32": dict(dtype=F16, bias=True, resid="f32"),
+    "f16_quick_gelu": dict(dtype=F16, bias=True, gelu=2),
+    "f16_quick_gelu_no_bias": dict(dtype=F16, gelu=2),
+    "f16_bias_alpha": dict(dtype=F16, bias=True, alpha=0.125),
+    "f16_patch_store": dict(dtype=F16, seg=(576, 577)),
+}
+TOWER_SHAPES = [(m, n) for m in (1, 129, 1731, 36864 + 64) for n in (1024, 4096)]
+PATCH_SHAPES = [(576 * crops, n) for crops in (1, 3, 64) for n in (1024, 4096)]     # the patch GEMM's rows are whole crops
+TOWER_CASES = [(kind, m, n) for kind, kw in TOWER_KINDS.items() for m, n in (PATCH_SHAPES if "seg" in kw else TOWER_SHAPES)]
+
+
+@pytest.fixture(scope="module")
+def ct():
+    return _lib("libtokenpacker_b200_clip_tower_hooks.so", {
+        "tpc_gemm_resid": [p, i64, p, i64, p, i64, i64, i64, i64, p, p, i64, i32, i32, i32, p]})
+
+
+@pytest.fixture(scope="module")
+def ct16():
+    return _lib("libtokenpacker_b200_clip_tower_f16_hooks.so", {
+        "tpc_gemm_f16": [p, i64, p, i64, p, i64, i64, i64, i64, p, p, i64, i32, i32, i32, C.c_float, i32, i32, i32, p]})
+
+
+def _tower_gemm(ct, ct16, kw, a, b, bias, r, m, n, k, mode):
+    """C of tpc_gemm_resid / tpc_gemm_f16 in a NaN frame of GUARD rows above and below and 64 columns to the right: returns the frame"""
+    dtype = kw["dtype"]
+    seg_len, seg_stride = kw.get("seg", (0, 0))
+    rows = m if seg_len == 0 else m // seg_len * seg_stride
+    frame = torch.full((rows + 2 * GUARD, n + 64), float("nan"), dtype=dtype, device=DEV)
+    c = frame[GUARD:GUARD + rows, :n]
+    ldr, resid_f32 = (0, 0) if r is None else (r.stride(0), int(r.dtype == torch.float32))
+    gelu = kw.get("gelu", 0)
+    if dtype == BF:
+        st = ct.tpc_gemm_resid(_ptr(a), k, _ptr(b), k, _ptr(c), n + 64, m, n, k, _ptr(bias), _ptr(r), ldr, resid_f32, gelu, mode, None)
+    else:
+        st = ct16.tpc_gemm_f16(_ptr(a), k, _ptr(b), k, _ptr(c), n + 64, m, n, k, _ptr(bias), _ptr(r), ldr, resid_f32, gelu, 0,
+                               kw.get("alpha", 1.0), seg_len, seg_stride, mode, None)
+    assert st == 0
+    torch.cuda.synchronize()
+    guards = [frame[:GUARD], frame[GUARD + rows:], frame[:, n:]]
+    if seg_len != 0:
+        guards.append(c.view(m // seg_len, seg_stride, n)[:, seg_len:])      # the rows between the segments are never written
+    assert all(bool(torch.isnan(x.float()).all()) for x in guards)
+    return frame
+
+
+@pytest.mark.parametrize("kind,m,n", TOWER_CASES)
+def test_tower_epilogue_same_bits_as_one_cta(ct, ct16, kind, m, n):
+    """The tower's epilogue kinds on the pair kernel (slabs written from the wgmma fragments) store the one-CTA kernel's bits, NaN
+    guards included.  The residual's row stride is wider than N."""
+    kw = TOWER_KINDS[kind]
+    dtype, k = kw["dtype"], 320
+    g = torch.Generator(device=DEV).manual_seed(401 + m + n)
+    a = torch.randn(m, k, generator=g, device=DEV).to(dtype)
+    b = (torch.randn(n, k, generator=g, device=DEV) * 0.05).to(dtype)
+    bias = torch.randn(n, generator=g, device=DEV) if kw.get("bias") else None
+    r = None
+    if "resid" in kw:
+        r = torch.randn(m, n + 8, generator=g, device=DEV) * 4
+        r = (r if kw["resid"] == "f32" else r.to(dtype))[:, :n]
+    one, pair = (_tower_gemm(ct, ct16, kw, a, b, bias, r, m, n, k, mode) for mode in (1, 2))
+    assert pair.view(torch.int16).equal(one.view(torch.int16)), "one-CTA and pair kernels differ"

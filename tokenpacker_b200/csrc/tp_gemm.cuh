@@ -17,12 +17,13 @@
 // CTA = 384 threads, persistent over output tiles:
 //   warps 0-7   two MMA + epilogue warpgroups, one per 64-row block of the CTA's 128 rows: one wgmma m64nNk16 per k16 step over
 //               the whole N-column tile (N/2 fp32 accumulators per thread), so each warpgroup reads its A block once and the B tile
-//               once per k-step; then the epilogue on the same registers.  Pair-kernel tiles stored through TMA (not the tower's):
-//               fused per-row / per-column math on the fragments in place, stmatrix into the swizzled shared-memory slabs
-//               (epilogue_tile_frag).  Everything else (KV-attention, direct global stores, the one-CTA kernel, the tower): each
-//               warp turns its fragments into thread == output row form (lanes 0-15: column half 0, lanes 16-31: column half 1 of
-//               the warp's 16 rows) through a 2 KiB shared-memory transpose (32 columns at a time), fused per-row / per-column
-//               math, swizzled shared-memory slabs (16-byte stores) or direct 16-byte global stores
+//               once per k-step; then the epilogue on the same registers.  Pair-kernel tiles stored through TMA (every
+//               instantiation): fused per-row / per-column math on the fragments in place, stmatrix into the swizzled shared-memory
+//               slabs (epilogue_tile_frag, the only slab writer).  Tiles with direct global stores (the one-CTA kernel; the pair
+//               kernel's scattered segment rows and fp32 outputs) and KV-attention tiles: each warp turns its fragments into
+//               thread == output row form (lanes 0-15: column half 0, lanes 16-31: column half 1 of the warp's 16 rows) through a
+//               2 KiB shared-memory transpose (32 columns at a time), then fused per-row / per-column math and 16-byte global stores
+//               (epilogue_tile) or the window softmax (attn_scores / attn_pv)
 //   warps 8, 9  store warps of the pair kernel (one per column half): wait for a finished slab on an mbarrier, issue its TMA
 //               store(s), hand the buffer back, and — for GEMMs that other GEMMs of the same launch depend on — publish each
 //               finished tile to a global counter.  The epilogue warps never wait for a store.
@@ -206,18 +207,10 @@ __device__ __forceinline__ void mma_tile(float (&acc)[2][kN * kRowBlocks / 4], c
 }
 
 // ------------------------------------------------------------------------------------------------
-// Shared epilogue for one 128-row x kTileN-column accumulator tile held in the registers of the CTA's two MMA warpgroups.
-//   acc      : this warpgroup's (= 64-row block's) wgmma accumulators, [column half][fragment registers of the half]
-//   scratch  : shared address of this warp's transpose scratch (kScratchBytesPerWarp)
-//   row      : global output row of this thread (tile row rloc = epi_row(wg, quarter, lane))
-//   col_tile0: global column of the tile's first column
-//   half     : the column half this thread owns (epi_half(lane))
-//   s_col    : shared staging for this tile's col_a / col_b slices, col_slot layout (already filled + synced)
-// ------------------------------------------------------------------------------------------------
-// Output staging for TMA stores: each column half of the tile owns two 16 KiB buffers holding a 128-row x 64-col slab in the
-// 128B-swizzled layout, 16 rows of it from each of the 8 epilogue warps (the 16 lanes of the warp that own that half); a slab is
-// written with conflict-free 16-byte st.shared, then ONE thread hands it
-// to the TMA unit (full 128-byte row segments instead of 16-byte scattered stores: less L1/L2 work and less power).
+// Output staging for the pair kernel's TMA stores: each column half of the tile owns two 16 KiB buffers holding a 128-row x 64-col
+// slab in the 128B-swizzled layout, 16 rows of it from each of the 8 epilogue warps.  epilogue_tile_frag writes a slab with stmatrix
+// and hands it over with one mbarrier arrive per warp; the half's store warp sends it to the TMA unit (full 128-byte row segments
+// instead of 16-byte scattered stores: less L1/L2 work and less power).
 constexpr int kMaxPeers = 8;
 // Fused all-gather: tensor maps of the SAME output slot in every peer GPU's gathered buffer (peer-mapped over NVLink);
 // each finished slab is TMA-stored to all of them instead of to one local matrix.
@@ -229,16 +222,9 @@ struct PeerStores {
   int whole;                 // 1: the whole-segment maps m[.][kBoxLevels + k - 1] (k segments) are valid (seg_len <= 128)
 };
 
-struct OutStage {
-  uint8_t* buf;              // this half's 2 x 16 KiB staging buffers (nullptr: direct 16-byte global stores)
-  uint64_t* full_bar;        // [2] slab written (count 8: one arrive per epilogue warp, from its lanes of the half) -> store warp
-  uint64_t* empty_bar;       // [2] slab's TMA store has finished reading the buffer (count 1, store warp) -> epilogue warps
-  uint32_t slab_seq;         // running slab number of this half (buffer = seq % 2, mbarrier phase = seq / 2)
-};
-// Output slab = 128 rows x 64 columns of bf16: 128-byte rows in TMA's SWIZZLE_128B layout.
+// Output slab = 128 rows x 64 columns of 16-bit values: 128-byte rows in TMA's SWIZZLE_128B layout.
 constexpr int kSlabCols = 64;
 constexpr int kSlabRowBytes = kSlabCols * 2;
-constexpr int kChunksPerSlab = kSlabCols / 32;
 constexpr int kOutSlabBytes = 128 * kSlabRowBytes;
 
 // Shared staging of a tile's per-column vectors: [col_a | col_b] x [column half 0 | kColPad | column half 1 | kColPad] floats.
@@ -275,8 +261,18 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
   rstd = rsqrtf(__fadd_rn(var, eps));
 }
 
+// ------------------------------------------------------------------------------------------------
+// Direct-store epilogue for one 128-row x kTileN-column accumulator tile held in the registers of the CTA's two MMA warpgroups: the
+// one-CTA kernel's tiles, and the pair kernel's tiles without TMA stores (scattered segment rows, fp32 output and split-K slices).
+// Each warp turns its fragments into thread == output row form through the transpose scratch, then stores 16 bytes at a time.
+//   acc      : this warpgroup's wgmma accumulators, [column half (pair kernel) | 64-row block (one-CTA kernel)][fragment registers]
+//   scratch  : shared address of this warp's transpose scratch (kScratchBytesPerWarp)
+//   row      : global output row of this thread (epi_row / epi_row_1cta)
+//   col_tile0: global column of the tile's first column
+//   half     : the column half this thread owns
+//   s_col    : shared staging for this tile's col_a / col_b slices, col_slot layout (already filled + synced)
 // kTower: the CLIP tower's instantiations (bias, bf16 or fp32 residual add, quick_gelu, alpha, fp32 output) — and none of the
-// projector's LayerNorm fold, row statistics, dual / window-major outputs, so that neither set of instantiations carries the other's registers.
+// projector's LayerNorm fold and row statistics, so that neither set of instantiations carries the other's registers.
 // kF16 (tower only): the same with an f16 residual and f16 output (one __floats2half2_rn rounding).
 // kSubPairs: packed column pairs (2 columns each) that go through every step together: each run-time option is ONE warp-uniform
 // branch around a basic block of kSubPairs independent dependency chains for the scheduler to interleave (more chains, more
@@ -284,8 +280,7 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
 // the 216-register limit.
 template <int kTileN, bool kTower = false, bool kF16 = false, int kSubPairs = 8>
 __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int N, const float (&acc)[2][kTileN / 4], uint32_t scratch,
-                                              int row, int rloc, int col_tile0, int half, const float* s_col, const OutStage& out,
-                                              long long c_extra = 0) {
+                                              int row, int col_tile0, int half, const float* s_col, long long c_extra = 0) {
   constexpr int kColsPerHalf = kTileN / 2;
   constexpr int kChunks = kColsPerHalf / 32;
   const bool ln_fold = !kTower && ep.col_a != nullptr;
@@ -308,7 +303,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
   float* c_row32 = reinterpret_cast<float*>(ep.c) + c_extra + dst_row * ep.ldc;     // out_f32 only (c_extra: split-K slice)
   const uint32_t sa_addr = smem_u32(s_col + col_slot<kTileN>(0, half * kColsPerHalf));
   const uint32_t sb_addr = smem_u32(s_col + col_slot<kTileN>(1, half * kColsPerHalf));
-  const uint32_t out_addr = out.buf != nullptr ? smem_u32(out.buf) : 0u;
 
   float s1 = 0.f, s2 = 0.f, shift = 0.f;     // statistics of (y - shift), shift = the block's first value: sums stay small
   const bool do_stats = !kTower && ep.stats_out != nullptr;
@@ -319,16 +313,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
   for (int chunk = 0; chunk < kChunks; ++chunk) {
     acc_chunk(acc, chunk, scratch, r);
     const int col0 = col_tile0 + half * kColsPerHalf + chunk * 32;
-    // dual output: every 64-column slab exists twice — pre-activation (even slab number, buffer 0) and activation (odd, buffer 1)
-    const bool dual = !kTower && ep.dual != 0 && out.buf != nullptr;
-    const uint32_t slab_pre = out.slab_seq + 2u * static_cast<uint32_t>(chunk / kChunksPerSlab);
-    const uint32_t slab_q = dual ? slab_pre + 1u : out.slab_seq + static_cast<uint32_t>(chunk / kChunksPerSlab);
-    const uint32_t slab_buf = slab_q & 1u;
-    if (out.buf != nullptr && (chunk % kChunksPerSlab) == 0) {
-      // the TMA store that last used this staging buffer must have finished READING it (signalled by the store warp)
-      if (dual) mbar_wait(&out.empty_bar[slab_pre & 1u], ((slab_pre >> 1) & 1u) ^ 1u);
-      mbar_wait(&out.empty_bar[slab_buf], ((slab_q >> 1) & 1u) ^ 1u);
-    }
     if (col0 < N) {        // N is a multiple of 32 (checked on the host) -> whole chunk in or out
 #pragma unroll
       for (int sub = 0; sub < 16 / kSubPairs; ++sub) {
@@ -352,22 +336,6 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
             const float4 b = lds_f4(sb4 + q * 16);
             v[2 * q] = add2(v[2 * q], pk2(b.x, b.y));
             v[2 * q + 1] = add2(v[2 * q + 1], pk2(b.z, b.w));
-          }
-        }
-        if (dual) {        // the pre-activation slab (same swizzled position in the other staging buffer)
-          const uint32_t row_pre = out_addr + static_cast<uint32_t>((slab_pre & 1u) * kOutSlabBytes + rloc * kSlabRowBytes);
-          const int swz_pre = rloc & 7;
-#pragma unroll
-          for (int g = 0; g < kSubPairs / 4; ++g) {
-            uint32_t w[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              float lo, hi;
-              upk2(v[4 * g + j], lo, hi);
-              w[j] = pack_bf16x2(lo, hi);
-            }
-            const int ci = (chunk % kChunksPerSlab) * 4 + sub * (kSubPairs / 4) + g;
-            sts_u4(row_pre + static_cast<uint32_t>((ci ^ swz_pre) << 4), w[0], w[1], w[2], w[3]);
           }
         }
         if constexpr (kTower) {
@@ -420,17 +388,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
             s2 = fmaf(y0, y0, fmaf(y1, y1, s2));
           }
         }
-        if (out.buf != nullptr) {
-          // 16-byte piece index inside the slab row, XOR-swizzled like TMA's SWIZZLE_128B does for 128-byte rows: with (row & 7),
-          // address bits [7,10) folded into bits [4,7)
-          const uint32_t row_base = out_addr + static_cast<uint32_t>(slab_buf * kOutSlabBytes + rloc * kSlabRowBytes);
-          const int swz = rloc & 7;
-#pragma unroll
-          for (int g = 0; g < kSubPairs / 4; ++g) {
-            const int ci = (chunk % kChunksPerSlab) * 4 + sub * (kSubPairs / 4) + g;
-            sts_u4(row_base + static_cast<uint32_t>((ci ^ swz) << 4), pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-          }
-        } else if (row_ok) {
+        if (row_ok) {
           if (ep.out_f32) {
 #pragma unroll
             for (int g = 0; g < kSubPairs / 2; ++g) {
@@ -447,29 +405,15 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
         }
       }
     }
-    if (chunk == kChunks - 1 && !kTower && ep.stats_out != nullptr && row_ok) {
-      // statistics are final once the last chunk's values exist; written BEFORE the last slab is handed over so that the store
-      // warp's tile-done release (dependent GEMMs of the same launch read them) covers these stores too
-      const int slot = (col_tile0 + half * kColsPerHalf) / kColsPerHalf;
-      long long srow = row;
-      if (!kTower && ep.wm_s != 0) srow = window_major_row(row, ep.wm_s);
-      if (slot < ep.stats_out_slots) {
-        // (mean, M2) of this 128-column block: mean = shift + s1/n, M2 = s2 - s1^2/n  (deviations from `shift` are O(std): no cancellation)
-        constexpr float inv_n = 1.0f / kColsPerHalf;
-        const float dm = __fmul_rn(s1, inv_n);
-        reinterpret_cast<float2*>(ep.stats_out)[srow * ep.stats_out_slots + slot] =
-            make_float2(__fadd_rn(shift, dm), fmaxf(fmaf(-s1, dm, s2), 0.f));
-      }
-    }
-    if (out.buf != nullptr && (chunk % kChunksPerSlab) == kChunksPerSlab - 1) {
-      // slab complete: make the generic-proxy writes visible to the async proxy, then one arrive per warp and column half hands
-      // it to the store warp
-      fence_proxy_async_smem();
-      __syncwarp();
-      if ((lane_id() & 15u) == 0) {
-        if (dual) mbar_arrive(&out.full_bar[slab_pre & 1u]);
-        mbar_arrive(&out.full_bar[slab_buf]);
-      }
+  }
+  if (do_stats && row_ok) {
+    const int slot = (col_tile0 + half * kColsPerHalf) / kColsPerHalf;
+    if (slot < ep.stats_out_slots) {
+      // (mean, M2) of this 128-column block: mean = shift + s1/n, M2 = s2 - s1^2/n  (deviations from `shift` are O(std): no cancellation)
+      constexpr float inv_n = 1.0f / kColsPerHalf;
+      const float dm = __fmul_rn(s1, inv_n);
+      reinterpret_cast<float2*>(ep.stats_out)[static_cast<long long>(row) * ep.stats_out_slots + slot] =
+          make_float2(__fadd_rn(shift, dm), fmaxf(fmaf(-s1, dm, s2), 0.f));
     }
   }
 }
@@ -639,31 +583,44 @@ __device__ __forceinline__ void col_vectors_ready() {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Pair kernel, tiles stored through the TMA slabs (not the tower's instantiations): the epilogue works on the wgmma m64n256
-// fragments where they are, with no transpose.  Lane (g = lane / 4, q = lane % 4) of a warp holds rows g and g + 8 of the warp's 16
-// rows, columns 8 j + 2 q, +1 of both column halves; every value goes through the same explicit fma / add / mul sequence as in
-// epilogue_tile, so the bits do not depend on which thread computes them.  The packed bf16 pairs are already in the m8n8 matrix
-// fragment form: stmatrix writes each 8 x 8 block's rows to their 128B-swizzled slab positions.  The warp writes both column halves,
-// slab by slab with the halves interleaved so that both store warps stay busy, and hands each half-slab over with one arrive.
+// Pair kernel, tiles stored through the TMA slabs (every instantiation): the epilogue works on the wgmma m64n256 fragments where
+// they are, with no transpose.  Lane (g = lane / 4, q = lane % 4) of a warp holds rows g and g + 8 of the warp's 16 rows, columns
+// 8 j + 2 q, +1 of both column halves; every value goes through the same explicit fma / add / mul sequence as in epilogue_tile, so
+// the bits do not depend on which thread computes them.  The packed 16-bit pairs are already in the m8n8 matrix fragment form:
+// stmatrix writes each 8 x 8 block's rows to their 128B-swizzled slab positions.  The warp writes both column halves, slab by slab
+// with the halves interleaved so that both store warps stay busy, and hands each half-slab over with one arrive.
 //   Row statistics keep epilogue_tile's order (sequential over the 128 rounded columns of a row and half): once both halves of a
 // slab are written, lane l re-reads row l % 16, column half l / 16 of it in column order — before the next slab is written, which
 // with dual output reuses the same activation buffer; the last slab of each half is handed over only once the statistics are
 // stored, so that the store warp's tile-done release covers them.
+//   kTower / kF16 as in epilogue_tile: the tower's residual is read at the lane's own fragment positions (one 4-byte load per
+// 16-bit pair, one 8-byte load per fp32 pair); the projector's LayerNorm fold, row statistics, dual output and erf GELU are
+// compiled out of the tower's instantiations.
 //   acc: [column half][fragment registers]; rloc_w0 / row_w0: tile row / global row of the warp's first row; s_out: the [2 halves]
 // [kOutBufs] slabs; full_bar / empty_bar: [2 halves][kOutBufs]; slab_seq: running slab number (both halves share it).
 // ------------------------------------------------------------------------------------------------
-template <int kOutBufs>
-__device__ __forceinline__ void epilogue_tile_frag(const GemmEpilogue& ep, int M, const float (&acc)[2][64], int row_w0, int rloc_w0,
+template <int kOutBufs, bool kTower = false, bool kF16 = false>
+__device__ __forceinline__ void epilogue_tile_frag(const GemmEpilogue& ep, int M, int N, const float (&acc)[2][64], int row_w0, int rloc_w0,
                                                    int col_tile0, const float* s_col, uint8_t* s_out, uint64_t* full_bar,
                                                    uint64_t* empty_bar, uint32_t slab_seq) {
   static_assert(kOutBufs == 2, "slab numbering: buffer = seq % 2");
   constexpr int kColsPerHalf = 128;
   const uint32_t lane = lane_id();
   const uint32_t g = lane >> 2, q = lane & 3u;
-  const bool ln_fold = ep.col_a != nullptr;
-  const bool dual = ep.dual != 0;
+  const bool ln_fold = !kTower && ep.col_a != nullptr;
+  const bool dual = !kTower && ep.dual != 0;
   const bool scale = ep.alpha != 1.0f;
-  const bool do_stats = ep.stats_out != nullptr;
+  const bool do_stats = !kTower && ep.stats_out != nullptr;
+  // the tower's residual rows g and g + 8 (nullptr: no residual, or the row is past M)
+  const uint8_t* resid_row[2] = {nullptr, nullptr};
+  if constexpr (kTower) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = row_w0 + static_cast<int>(g) + 8 * r;
+      if (ep.resid != nullptr && row < M)
+        resid_row[r] = static_cast<const uint8_t*>(ep.resid) + static_cast<long long>(row) * ep.ldr * (ep.resid_f32 ? 4 : 2);
+    }
+  }
   uint64_t rstd2[2], nmu2[2];
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
@@ -715,6 +672,20 @@ __device__ __forceinline__ void epilogue_tile_frag(const GemmEpilogue& ep, int M
 #pragma unroll
             for (int r = 0; r < 2; ++r) v[2 * jj + r] = add2(pk2(acc[h][4 * j + 2 * r], acc[h][4 * j + 2 * r + 1]), b2);
           }
+          if constexpr (kTower) {   // one rounding of acc + bias + R: the residual add of a CLIP layer
+            const long long col = col_tile0 + h * kColsPerHalf + 8 * j + 2 * static_cast<int>(q);
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              if (resid_row[r] == nullptr || col >= N) continue;
+              if (ep.resid_f32) {
+                const float2 x = *reinterpret_cast<const float2*>(resid_row[r] + col * 4);
+                v[2 * jj + r] = add2(v[2 * jj + r], pk2(x.x, x.y));
+              } else {
+                const uint32_t x = *reinterpret_cast<const uint32_t*>(resid_row[r] + col * 2);
+                v[2 * jj + r] = add2(v[2 * jj + r], pk2(x2_lo<kF16>(x), x2_hi<kF16>(x)));
+              }
+            }
+          }
         }
         // 16-byte piece of the slab row: groups 2 x + m_grp, XOR-swizzled like TMA's SWIZZLE_128B
         const uint32_t piece = ((2u * static_cast<uint32_t>(x) + m_grp) ^ (lane & 7u)) << 4;
@@ -728,7 +699,12 @@ __device__ __forceinline__ void epilogue_tile_frag(const GemmEpilogue& ep, int M
           }
           stmatrix_x4(half_addr + (slab_pre & 1u) * kOutSlabBytes + piece, w[0], w[1], w[2], w[3]);
         }
-        if (ep.gelu) {
+        if constexpr (kTower) {
+          if (ep.gelu == 2) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) v[k] = quick_gelu_pk(v[k]);
+          }
+        } else if (ep.gelu) {
 #pragma unroll
           for (int k = 0; k < 4; ++k) v[k] = gelu_erf_pk(v[k]);
         }
@@ -740,7 +716,7 @@ __device__ __forceinline__ void epilogue_tile_frag(const GemmEpilogue& ep, int M
         for (int k = 0; k < 4; ++k) {
           float lo, hi;
           upk2(v[k], lo, hi);
-          w[k] = pack_bf16x2(lo, hi);
+          w[k] = pack_x2<kF16>(lo, hi);
         }
         stmatrix_x4(half_addr + (slab_q & 1u) * kOutSlabBytes + piece, w[0], w[1], w[2], w[3]);
       }
@@ -893,9 +869,7 @@ tp_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       stage_col_vectors<kBlockN>(ep, N, n_blk * kBlockN, s_col, epi_tid, true);
       mma_tile<kN, 2, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, 0, Cfg::kABytes + half * kN * kBlockK * 2, full_bar, empty_bar, kStages, stage,
                                   phase, num_k_blocks);
-      const OutStage no_stage{nullptr, nullptr, nullptr, 0u};
-      epilogue_tile<kBlockN, kTower, kF16>(ep, M, N, acc, scratch, m_blk * kBlockM + rloc, rloc, n_blk * kBlockN, half, s_col,
-                                           no_stage);
+      epilogue_tile<kBlockN, kTower, kF16>(ep, M, N, acc, scratch, m_blk * kBlockM + rloc, n_blk * kBlockN, half, s_col);
     }
   }
 }
@@ -1165,18 +1139,15 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       else
         mma_tile<kTileN, 1, 0, 0, kF16>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, n_kb);
       col_vectors_ready();
-      if (!kTower && pr.use_tma_store) {
+      if (pr.use_tma_store) {
         const int rloc_w0 = 64 * wg + 16 * (warp_idx & 3);
-        epilogue_tile_frag<Cfg::kOutBufs>(pr.ep, pr.M, acc, row_tile0 + rloc_w0, rloc_w0, t.n_blk * kTileN, s_col, s_out, slab_full_bar,
-                                          slab_empty_bar, slab_seq);
+        epilogue_tile_frag<Cfg::kOutBufs, kTower, kF16>(pr.ep, pr.M, pr.N, acc, row_tile0 + rloc_w0, rloc_w0, t.n_blk * kTileN, s_col, s_out,
+                                                        slab_full_bar, slab_empty_bar, slab_seq);
         slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);                        // slabs per tile and column half
-        continue;
+      } else {
+        epilogue_tile<kTileN, kTower, kF16, 4>(pr.ep, pr.M, pr.N, acc, scratch, row, t.n_blk * kTileN, half, s_col,
+                                               static_cast<long long>(t.split) * pr.c_split_stride);
       }
-      const OutStage out{pr.use_tma_store ? s_out + half * Cfg::kOutBufs * kOutSlabBytes : nullptr, slab_full_bar + half * Cfg::kOutBufs,
-                         slab_empty_bar + half * Cfg::kOutBufs, slab_seq};
-      if (pr.use_tma_store) slab_seq += (kTileN / 2 / kSlabCols) * (pr.ep.dual ? 2 : 1);     // slabs per tile and column half
-      epilogue_tile<kTileN, kTower, kF16, 4>(pr.ep, pr.M, pr.N, acc, scratch, row, rloc, t.n_blk * kTileN, half, s_col, out,
-                                    static_cast<long long>(t.split) * pr.c_split_stride);
     }
   } else {
     setmaxnreg_dec<kAuxRegs>();
