@@ -4,7 +4,7 @@ There is deliberately no fallback: if the shared library is missing the import f
 Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
 include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h, include/tokenpacker_b200_clip_tower.h,
 include/tokenpacker_b200_clip_tower_f16.h, include/tokenpacker_b200_clip_tower_train.h, include/tokenpacker_b200_clip_tower_ckpt.h,
-include/tokenpacker_b200_clip_tower_embed.h, include/tokenpacker_b200_jpeg.h and include/tokenpacker_b200_png.h one to one.
+include/tokenpacker_b200_clip_tower_embed.h, include/tokenpacker_b200_clip_tower_crop_grad.h, include/tokenpacker_b200_jpeg.h and include/tokenpacker_b200_png.h one to one.
 """
 from __future__ import annotations
 
@@ -235,6 +235,27 @@ CLIP_TOWER_EMBED_SIGNATURES = {
 }
 
 
+# the same for include/tokenpacker_b200_clip_tower_crop_grad.h (gradients to the crops and through the HD tiling to the images)
+TP_CROP_GRAD_BF16 = 0
+TP_CROP_GRAD_F32 = 1
+
+
+class TpHdImageGrad(C.Structure):
+    """tp_hd_image_grad: where tp_hd_tile_batch_backward writes one image's gradient, and where its inverse-tap tables are."""
+    _fields_ = [("d_image", C.c_void_p), ("row_taps", C.c_int64), ("col_taps", C.c_int64), ("thumb_row_taps", C.c_int64),
+                ("thumb_col_taps", C.c_int64)]
+
+
+CROP_GRAD_SIGNATURES = {
+    "tp_clip_tower_backward_crops": (C.c_int, [C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_void_p, C.c_int64, C.c_int,
+                                               C.POINTER(C.c_void_p), C.POINTER(TpClipTowerLayerGrads), C.POINTER(TpClipTowerEmbedGrads),
+                                               C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "tp_hd_tile_batch_backward_plan": (C.c_int, [C.POINTER(TpHdImage), C.c_int64, C.POINTER(C.c_void_p), C.POINTER(TpHdImageGrad),
+                                                 C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "tp_hd_tile_batch_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+}
+
+
 # the same for include/tokenpacker_b200_jpeg.h (baseline JPEG files decoded on the GPU, bit for bit as PIL)
 class TpJpegImage(C.Structure):
     """tp_jpeg_image: one row of the decode plan."""
@@ -318,7 +339,7 @@ def _load():
     for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
                                       **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES,
                                       **CLIP_TOWER_TRAIN_SIGNATURES, **CLIP_TOWER_CKPT_SIGNATURES,
-                                      **CLIP_TOWER_EMBED_SIGNATURES, **JPEG_SIGNATURES, **PNG_SIGNATURES}.items():
+                                      **CLIP_TOWER_EMBED_SIGNATURES, **CROP_GRAD_SIGNATURES, **JPEG_SIGNATURES, **PNG_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly
         fn.restype = restype
         fn.argtypes = argtypes

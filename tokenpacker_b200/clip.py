@@ -51,7 +51,9 @@ def clip_preprocess_batch(images, aspect_ratio: str = "pad", dtype=torch.float32
     for "CHW" (torchvision.io.decode_image); sizes may differ, and views are read through their strides, not copied.
     aspect_ratio: "pad" (``image_aspect_ratio == 'pad'``) or "square" (the default ``'square'``: the processor alone).
     dtype: torch.float32, or torch.bfloat16 (the tower's dtype; equal to the float32 output .to(torch.bfloat16), bit for bit).
-    Returns [B, 3, 336, 336] in dtype, in the order of the images: the processor's ``pixel_values``, bit for bit in float32."""
+    Returns [B, 3, 336, 336] in dtype, in the order of the images: the processor's ``pixel_values``, bit for bit in float32.  Not
+    differentiable: the inputs are integer pixels and the resize is PIL's integer arithmetic; gradients to the pixels start at these
+    crops (``crops.requires_grad_()`` with ``CLIPVisionTowerB200.input_grad``)."""
     mode = _mode(aspect_ratio)
     images, device, sizes, sources = _u8_sources(images, dtype, layout)
     b = len(images)

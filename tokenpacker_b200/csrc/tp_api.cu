@@ -17,6 +17,7 @@
 #include "../../include/tokenpacker_b200_clip_tower_train.h"
 #include "../../include/tokenpacker_b200_clip_tower_ckpt.h"
 #include "../../include/tokenpacker_b200_clip_tower_embed.h"
+#include "../../include/tokenpacker_b200_clip_tower_crop_grad.h"
 #include "../../include/tokenpacker_b200_clip_u8.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"
@@ -1923,5 +1924,6 @@ int tp_hd_fill_separators(void* out, int hidden, const int64_t* sep_rows, int64_
 #include "tp_clip_tower_train.inl"
 #include "tp_clip_tower_ckpt.inl"
 #include "tp_clip_tower_embed.inl"
+#include "tp_clip_tower_crop_grad.inl"
 #include "tp_jpeg.inl"
 #include "tp_png.inl"

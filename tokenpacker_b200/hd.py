@@ -54,7 +54,8 @@ def n_crops(hb: int, wb: int) -> int:
 
 def hd_tile(image: torch.Tensor, patch_num: int = 9):
     """train.py:695-731 on the GPU.  image: float32 CUDA tensor [1,3,h,w] (or [3,h,w]), already normalised.
-    Returns (crops [hb*wb(+1), 3, 336, 336] float32, h_block, w_block)."""
+    Returns (crops [hb*wb(+1), 3, 336, 336] float32, h_block, w_block).  Under grad mode, when the image requires grad, the crops are
+    attached to autograd and their backward (tp_hd_tile_batch_backward) gives the image its gradient, bit for bit as hd_tile_batch's."""
     if image.dim() == 4:
         if image.shape[0] != 1:
             raise ValueError("one image per call: [1,3,h,w]")
@@ -66,11 +67,68 @@ def hd_tile(image: torch.Tensor, patch_num: int = 9):
     image = image.to(torch.float32).contiguous()
     h, w = int(image.shape[1]), int(image.shape[2])
     hb, wb = hd_grid(h, w, patch_num)
-    with torch.cuda.device(image.device):
-        crops = torch.empty((n_crops(hb, wb), 3, BLOCK, BLOCK), dtype=torch.float32, device=image.device)
-        stream = torch.cuda.current_stream(image.device).cuda_stream
-        check(lib.tp_hd_tile(image.data_ptr(), h, w, hb, wb, crops.data_ptr(), stream), "tp_hd_tile")
-    return crops, hb, wb
+
+    def launch(imgs):
+        with torch.cuda.device(image.device):
+            crops = torch.empty((n_crops(hb, wb), 3, BLOCK, BLOCK), dtype=torch.float32, device=image.device)
+            stream = torch.cuda.current_stream(image.device).cuda_stream
+            check(lib.tp_hd_tile(imgs[0].data_ptr(), h, w, hb, wb, crops.data_ptr(), stream), "tp_hd_tile")
+        return crops
+
+    if torch.is_grad_enabled() and image.requires_grad:
+        return _HdTileFunction.apply(launch, patch_num, image), hb, wb
+    return launch([image]), hb, wb
+
+
+def _tile_batch_backward(sizes, patch_num: int, d_crops: torch.Tensor):
+    """d images (fp32 [3, h, w] each) from the gradient of the crops of a tiling launch over images of these sizes
+    (tp_hd_tile_batch_backward_plan + tp_hd_tile_batch_backward, on the current stream of d_crops' device)."""
+    device = d_crops.device
+    d_crops = d_crops.to(torch.float32).contiguous()
+    b = len(sizes)
+    hs = (C.c_int64 * b)(*[h for h, _ in sizes])
+    ws = (C.c_int64 * b)(*[w for _, w in sizes])
+    hb, wb = (C.c_int * b)(), (C.c_int * b)()
+    nc = C.c_int64(0)
+    desc = (_lib.TpHdImage * b)()
+    check(lib.tp_hd_tile_batch_plan(hs, ws, None, b, int(patch_num), desc, None, hb, wb, C.byref(nc)), "tp_hd_tile_batch_plan")
+    if nc.value != d_crops.shape[0]:
+        raise ValueError(f"the images make {nc.value} crops, the gradient has {d_crops.shape[0]}")
+    d_images = [torch.empty((3, h, w), dtype=torch.float32, device=device) for h, w in sizes]
+    ptrs = (C.c_void_p * b)(*[t.data_ptr() for t in d_images])
+    words, most = C.c_int64(0), C.c_int64(0)
+    check(lib.tp_hd_tile_batch_backward_plan(desc, b, ptrs, None, None, C.byref(words), C.byref(most)), "tp_hd_tile_batch_backward_plan")
+    desc_bytes = C.sizeof(_lib.TpHdImage) * b
+    grad_off = (desc_bytes + 15) // 16 * 16
+    taps_off = (grad_off + C.sizeof(_lib.TpHdImageGrad) * b + 15) // 16 * 16
+    host = torch.empty(taps_off + max(words.value, 1) * 4, dtype=torch.uint8)
+    C.memmove(host.data_ptr(), C.addressof(desc), desc_bytes)
+    grads = (_lib.TpHdImageGrad * b).from_address(host.data_ptr() + grad_off)
+    check(lib.tp_hd_tile_batch_backward_plan(desc, b, ptrs, grads, C.cast(host.data_ptr() + taps_off, C.POINTER(C.c_int32)), C.byref(words),
+                                             C.byref(most)), "tp_hd_tile_batch_backward_plan")
+    with torch.cuda.device(device):
+        dev = host.to(device)
+        stream = torch.cuda.current_stream(device).cuda_stream
+        check(lib.tp_hd_tile_batch_backward(dev.data_ptr(), dev.data_ptr() + grad_off, dev.data_ptr() + taps_off, b, most.value,
+                                            d_crops.data_ptr(), stream), "tp_hd_tile_batch_backward")
+    return d_images
+
+
+class _HdTileFunction(torch.autograd.Function):
+    """The tiling block under autograd: the forward is ``launch(images)`` (tp_hd_tile or tp_hd_tile_batch, unchanged), the backward
+    its exact adjoint, tp_hd_tile_batch_backward.  images: float32 [3, h, w], contiguous."""
+
+    @staticmethod
+    def forward(ctx, launch, patch_num, *images):
+        ctx.sizes = [(int(im.shape[1]), int(im.shape[2])) for im in images]
+        ctx.patch_num = patch_num
+        return launch(images)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, d_crops):
+        d_images = _tile_batch_backward(ctx.sizes, ctx.patch_num, d_crops)
+        return (None, None) + tuple(d if need else None for d, need in zip(d_images, ctx.needs_input_grad[2:]))
 
 
 _STAGING: dict = {}
@@ -96,7 +154,10 @@ def hd_tile_batch(images, patch_num: int = 9, _return_launch: bool = False):
 
     images: sequence of float32 CUDA tensors [3,h,w] or [1,3,h,w] (already normalised), sizes may differ.
     Returns (crops [sum_i n_crops_i, 3, 336, 336] float32 in the reference's order — image by image, grid row-major, thumbnail
-    last —, h_block list, w_block list)."""
+    last —, h_block list, w_block list).
+    Under grad mode, when some image requires grad, the crops are attached to autograd: their backward is the exact adjoint of the
+    tiling block (tp_hd_tile_batch_backward: the bilinear resizes, the zero padding, the split and the thumbnail), deterministic,
+    and gives each image that requires grad its fp32 gradient.  Otherwise the launch is the same."""
     imgs = []
     for im in images:
         if im.dim() == 4:
@@ -114,8 +175,20 @@ def hd_tile_batch(images, patch_num: int = 9, _return_launch: bool = False):
     def launch(tables, _sources, crop_table, n, crops, stream):
         check(lib.tp_hd_tile_batch(tables, crop_table, n, crops.data_ptr(), stream), "tp_hd_tile_batch")
 
-    crops, hb, wb, (dev, _, table_off, n) = _run_tile_batch(imgs[0].device, [(int(im.shape[1]), int(im.shape[2])) for im in imgs],
-                                                             [im.data_ptr() for im in imgs], None, patch_num, torch.float32, imgs, launch)
+    sizes = [(int(im.shape[1]), int(im.shape[2])) for im in imgs]
+    if torch.is_grad_enabled() and any(im.requires_grad for im in imgs) and not _return_launch:
+        grids = []
+
+        def run(images):
+            crops, hb, wb, _ = _run_tile_batch(images[0].device, sizes, [im.data_ptr() for im in images], None, patch_num, torch.float32,
+                                               images, launch)
+            grids.append((hb, wb))
+            return crops
+
+        crops = _HdTileFunction.apply(run, patch_num, *imgs)
+        return crops, grids[0][0], grids[0][1]
+    crops, hb, wb, (dev, _, table_off, n) = _run_tile_batch(imgs[0].device, sizes, [im.data_ptr() for im in imgs], None, patch_num,
+                                                             torch.float32, imgs, launch)
     if _return_launch:
         # benchmark hook: (device tables, table offset, crop count) so that the kernel can be re-launched and timed on its own
         return crops, hb, wb, (dev, table_off, n)
@@ -229,7 +302,8 @@ def hd_preprocess_batch(images, patch_num: int = 9, dtype=torch.float32, layout:
     for "CHW" (torchvision.io.decode_image); sizes may differ, and views are read through their strides, not copied.
     dtype: torch.float32, or torch.bfloat16 (the tower's dtype; equal to the float32 crops .to(torch.bfloat16), bit for bit).
     Returns (crops [sum_i n_crops_i, 3, 336, 336] in dtype, h_block list, w_block list) in the reference's crop order.  The float32
-    crops have exactly the bits hd_tile_batch gives for the same images normalised on the host (norm_table)."""
+    crops have exactly the bits hd_tile_batch gives for the same images normalised on the host (norm_table).  Not differentiable: the
+    inputs are integer pixels and the arithmetic is PIL's; for gradients to the pixels, normalise on the host and use hd_tile_batch."""
     images, device, sizes, sources = _u8_sources(images, dtype, layout)
     table = _norm_table_on(device)
     out_dtype = 0 if dtype == torch.float32 else 1

@@ -28,6 +28,10 @@ recomputes the rest in the backward (include/tokenpacker_b200_clip_tower_ckpt.h)
 ``CLIPVisionTowerB200(model, trainable_layers=23, train_embeddings=True)`` trains the whole tower: below the 23 layers, pre_layrnorm, the
 class and position embeddings and the patch embedding get their gradients too (include/tokenpacker_b200_clip_tower_embed.h), with or
 without gradient checkpointing.  That is what the recipes that unfreeze the vision tower (``vision_tower.requires_grad_(True)``) need.
+
+``tower.input_grad = True`` backpropagates to the pixels: crops that require grad get their gradient (adversarial evaluation,
+attribution of packed tokens to image regions, pixel-space perturbation learning); with ``hd_tile_batch`` the gradient reaches the
+normalised images (INTEGRATION.md).
 """
 from __future__ import annotations
 
@@ -119,6 +123,76 @@ class _TowerTrainFunction(torch.autograd.Function):
         return (None,) * _NUM_FN_INPUTS + tuple(grads)
 
 
+class _TowerCropGradFunction(torch.autograd.Function):
+    """hidden_states 12 / 16 / 22 / 23 with the crops under autograd (``tower.input_grad``): the whole-tower training pair
+    (tp_clip_tower_forward_train_embed at 23 layers) and tp_clip_tower_backward_crops.  Inputs after the first five are the tower's
+    trainable parameters in _TowerTrainFunction's order; those that require grad get their gradients, every other layer only passes
+    its input gradient on.  ``images`` are the caller's crops: they are cast to bf16 here, so that fp32 crops receive the fp32 gradient
+    the kernels accumulate."""
+
+    @staticmethod
+    def forward(ctx, tower, images, packed, w, checkpoint, *params):
+        k, n, device = _lib.CLIP_TOWER_LAYERS, images.shape[0], images.device
+        x = images.to(torch.bfloat16)
+        if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
+            x = x.contiguous()
+        outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=torch.bfloat16, device=device) for _ in _OUT_LAYERS)
+        if checkpoint:
+            saved_bytes, ws_bytes = lib.tp_clip_tower_ckpt_saved_bytes(n, k), lib.tp_clip_tower_workspace_bytes(n)
+        else:
+            saved_bytes, ws_bytes = lib.tp_clip_tower_train_saved_bytes(n, k), lib.tp_clip_tower_train_workspace_bytes(n, k)
+        embed_bytes = lib.tp_clip_tower_embed_saved_bytes(n)
+        saved = torch.empty(saved_bytes, dtype=torch.uint8, device=device)
+        embed_saved = torch.empty(embed_bytes, dtype=torch.uint8, device=device)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            check(lib.tp_clip_tower_forward_train_embed(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), int(checkpoint), ptrs,
+                                                        saved.data_ptr(), saved_bytes, embed_saved.data_ptr(), embed_bytes, ws.data_ptr(),
+                                                        ws_bytes, stream), "tp_clip_tower_forward_train_embed")
+        ctx.w, ctx.saved, ctx.embed_saved, ctx.n, ctx.checkpoint = w, saved, embed_saved, n, checkpoint
+        ctx.trainable_layers, ctx.train_embeddings, ctx.params = tower.trainable_layers, tower.train_embeddings, params
+        ctx.crops_dtype = images.dtype
+        ctx.set_materialize_grads(False)
+        return outs
+
+    @staticmethod
+    def backward(ctx, *d_outs):
+        n, device = ctx.n, ctx.saved.device
+        d_outs = [None if g is None else g.to(torch.bfloat16).contiguous() for g in d_outs]
+        d_ptrs = (C.c_void_p * 4)(*[None if g is None else g.data_ptr() for g in d_outs])
+        grads = [torch.empty_like(p) if ctx.needs_input_grad[_NUM_FN_INPUTS + i] else None for i, p in enumerate(ctx.params)]
+        ptr = [None if g is None else g.data_ptr() for g in grads]
+        n_top = len(_lib.CLIP_TOWER_FIELDS) if ctx.train_embeddings else 0
+        per, first = len(_lib.CLIP_TOWER_LAYER_FIELDS), _lib.CLIP_TOWER_LAYERS - ctx.trainable_layers
+        g_structs = (_lib.TpClipTowerLayerGrads * _lib.CLIP_TOWER_LAYERS)()
+        for t in range(ctx.trainable_layers):
+            g_structs[first + t] = _lib.TpClipTowerLayerGrads(*ptr[n_top + t * per:n_top + (t + 1) * per])
+        e_struct = _lib.TpClipTowerEmbedGrads(*ptr[:n_top]) if n_top else _lib.TpClipTowerEmbedGrads()
+        f32 = ctx.crops_dtype == torch.float32
+        d_crops = None
+        if ctx.needs_input_grad[1]:
+            d_crops = torch.empty((n, 3, _IMAGE, _IMAGE), dtype=torch.float32 if f32 else torch.bfloat16, device=device)
+        k = _lib.CLIP_TOWER_LAYERS
+        ws_bytes = (lib.tp_clip_tower_ckpt_backward_workspace_bytes if ctx.checkpoint else lib.tp_clip_tower_backward_workspace_bytes)(n, k)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        with torch.cuda.device(device):
+            stream = torch.cuda.current_stream(device).cuda_stream
+            if d_crops is not None:
+                check(lib.tp_clip_tower_backward_crops(C.byref(ctx.w), ctx.saved.data_ptr(), ctx.embed_saved.data_ptr(), n, int(ctx.checkpoint),
+                                                       d_ptrs, g_structs, C.byref(e_struct), d_crops.data_ptr(),
+                                                       _lib.TP_CROP_GRAD_F32 if f32 else _lib.TP_CROP_GRAD_BF16, d_crops.stride(0),
+                                                       ws.data_ptr(), ws_bytes, stream), "tp_clip_tower_backward_crops")
+            else:
+                check(lib.tp_clip_tower_backward_embed(C.byref(ctx.w), ctx.saved.data_ptr(), ctx.embed_saved.data_ptr(), n, int(ctx.checkpoint),
+                                                       d_ptrs, g_structs, C.byref(e_struct), ws.data_ptr(), ws_bytes, stream),
+                      "tp_clip_tower_backward_embed")
+        if d_crops is not None and not f32 and ctx.crops_dtype != torch.bfloat16:
+            d_crops = d_crops.to(ctx.crops_dtype)
+        return (None, d_crops) + (None,) * (_NUM_FN_INPUTS - 2) + tuple(grads)
+
+
 def wants_gradient_checkpointing(vision_model: nn.Module) -> bool:
     """Whether the wrapped model asks for gradient checkpointing: some submodule has ``gradient_checkpointing`` truthy and is in
     training mode.  That is the condition under which transformers' own CLIPEncoder recomputes its layers
@@ -165,6 +239,10 @@ class CLIPVisionTowerB200(nn.Module):
     set ``requires_grad=False`` on those layers' parameters: the backward still runs through them (their input gradients), and skips
     their weight gradients.
 
+    input_grad: False (the default) or True; an attribute, like ``TokenPackerB200.input_grad``, not a constructor argument and not in
+    the state_dict, and refused with dtype=torch.float16 (the fp16 tower is forward only).  True: crops that require grad get their
+    gradient under grad mode (see ``hidden_states``).
+
     Gradient checkpointing has no switch of its own: the tower follows the wrapped model's (``gradient_checkpointing_enable()`` /
     ``_disable()``, see ``wants_gradient_checkpointing``).  Checkpointing trades time for memory and no property of the input decides
     between them, so the choice stays with the switch the model and the recipe that sets it already own; a second option here could
@@ -202,7 +280,20 @@ class CLIPVisionTowerB200(nn.Module):
         self._packed_key = None
         self._weights = None
         self._warned_dtype = False
+        self._input_grad = False
         self.register_load_state_dict_post_hook(lambda module, incompatible: module.invalidate_packed())
+
+    @property
+    def input_grad(self) -> bool:
+        return self._input_grad
+
+    @input_grad.setter
+    def input_grad(self, value: bool):
+        if not isinstance(value, bool):
+            raise ValueError(f"input_grad = {value!r}: expected True or False")
+        if value and self.dtype == torch.float16:
+            raise ValueError("input_grad needs the bf16 tower: the fp16 tower is forward only")
+        self._input_grad = value
 
     def invalidate_packed(self):
         """Drop the derived weight cache (call it after writing parameters through a ``.data`` alias: such writes change neither
@@ -292,12 +383,32 @@ class CLIPVisionTowerB200(nn.Module):
         bits as without it.  A graph keeps the mode it was built with.
         With train_embeddings (trainable_layers = 23), the embedding stage's five parameters count among the trainable ones above: read
         in place under the same conditions, each that requires grad gets its gradient, and the step keeps in addition the crops' patch
-        rows and the patch embedding's output (1.9 MB per crop), in both modes."""
+        rows and the patch embedding's output (1.9 MB per crop), in both modes.
+        With ``input_grad`` (bf16 tower), under grad mode and when the crops require grad: the step runs the whole-tower training pair
+        (all 23 layers and the embedding stage, include/tokenpacker_b200_clip_tower_crop_grad.h), the four hidden states are attached to
+        autograd, and the backward gives the crops their gradient (fp32 crops an fp32 gradient straight from the kernels' fp32 sums,
+        other crops a bf16 one in their dtype; crop views of any crop stride are read in place).  Parameters get gradients exactly as
+        above (those of the trainable layers and, with train_embeddings, of the embedding stage that require grad, with the bits the
+        step without input_grad gives); every other layer only passes its input gradient on, whatever its requires_grad says.  The
+        step keeps the saved sets of all 23 layers: about 23 x 20.1 MB per crop plus 1.86 MB per crop for the embedding stage, or with
+        gradient checkpointing 23 x 1.2 MB per crop plus 23 x 6.3 MB (and the 1.86 MB per crop).  Checkpointing follows
+        ``wants_gradient_checkpointing``, which needs the wrapped model in training mode: an attribution run on an eval-mode model keeps
+        the full saved sets."""
         if not isinstance(images, torch.Tensor) or images.dim() != 4 or tuple(images.shape[1:]) != (3, _IMAGE, _IMAGE):
             shape = tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__
             raise ValueError(f"expected crops [N,3,336,336], got {shape}")
         train_params = self._trainable_params() if torch.is_grad_enabled() else []
         train = any(p.requires_grad for p in train_params)
+        crop_grad = self._input_grad and torch.is_grad_enabled() and images.requires_grad
+        if crop_grad:
+            if not images.is_cuda:
+                raise RuntimeError("tokenpacker_b200 has no CPU path: crops must be CUDA tensors on an H100")
+            if images.shape[0] == 0:
+                raise ValueError("input_grad needs at least one crop")
+            with torch.cuda.device(images.device):
+                packed, (w, _) = self._packed_weights(images.device)
+                return _TowerCropGradFunction.apply(self, images, packed, self._live_weights(w, train_params, images.device),
+                                                    wants_gradient_checkpointing(self.vision_model), *train_params)
         if torch.is_grad_enabled() and (images.requires_grad or (self.trainable_layers == 0 and any(p.requires_grad for p in self._params()))):
             raise NotImplementedError("CLIPVisionTowerB200 is forward only (the tower is frozen in every TokenPacker recipe): run it under "
                                       "torch.no_grad(), or detach the crops and freeze the tower's parameters")
