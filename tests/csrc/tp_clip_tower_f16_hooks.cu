@@ -67,7 +67,9 @@ TP_API int tpc_layer_f16(const void* packed, const tp_clip_tower_weights* w, int
   uint8_t* W = static_cast<uint8_t*>(workspace);
   int* flags = reinterpret_cast<int*>(W + WL.flags);
   TP_CUDA(cudaMemsetAsync(flags, 0, static_cast<size_t>(WL.flags_per_layer) * 4, stream));
-  return run_clip_layer(static_cast<const uint8_t*>(packed), w, layer, x, x_out, W, WL, n, flags, dev.sms, stream, true);
+  const ClipPackedLayout PL = clip_packed_layout();
+  return run_clip_layer(static_cast<const uint8_t*>(packed) + PL.layer0 + layer * PL.layer_bytes, w, layer, x, x_out, W, WL, n, flags, dev.sms,
+                        stream, true);
 }
 
 // Status of a launch that mixes one bf16 and one f16 tower item (fc1 -> fc2 shapes, addresses that are never dereferenced): as a

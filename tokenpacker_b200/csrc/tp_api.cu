@@ -1922,7 +1922,6 @@ int tp_hd_fill_separators(void* out, int hidden, const int64_t* sep_rows, int64_
 
 #include "tp_clip_tower.inl"
 #include "tp_clip_tower_train.inl"
-#include "tp_clip_tower_ckpt.inl"
 #include "tp_clip_tower_embed.inl"
 #include "tp_clip_tower_crop_grad.inl"
 #include "tp_jpeg.inl"

@@ -49,44 +49,66 @@ _IMAGE = 336
 _OUT_LAYERS = (12, 16, 22, 23)
 
 
-_NUM_FN_INPUTS = 5                                      # _TowerTrainFunction's inputs before the parameters
+_NUM_FN_INPUTS = 6                                      # _TowerTrainFunction's inputs before the parameters
+
+
+def _train_step(checkpoint: bool, embed: bool, crop_grad: bool, n: int, k: int):
+    """The entry points and buffer sizes of a training step over n crops that runs the top k layers: (forward, backward, saved bytes,
+    forward workspace bytes, backward workspace bytes).  checkpoint: keep each layer's checkpoint (include/tokenpacker_b200_clip_tower_ckpt.h)
+    instead of its full saved set; embed: the whole tower, k = 23 and the embedding stage (include/tokenpacker_b200_clip_tower_embed.h);
+    crop_grad: the whole tower's backward gives the crops their gradient too (include/tokenpacker_b200_clip_tower_crop_grad.h)."""
+    if checkpoint:
+        names = ("tp_clip_tower_forward_ckpt", "tp_clip_tower_backward_ckpt")
+        sizes = (lib.tp_clip_tower_ckpt_saved_bytes(n, k), lib.tp_clip_tower_workspace_bytes(n),
+                 lib.tp_clip_tower_ckpt_backward_workspace_bytes(n, k))
+    else:
+        names = ("tp_clip_tower_forward_train", "tp_clip_tower_backward")
+        sizes = (lib.tp_clip_tower_train_saved_bytes(n, k), lib.tp_clip_tower_train_workspace_bytes(n, k),
+                 lib.tp_clip_tower_backward_workspace_bytes(n, k))
+    if embed:
+        names = ("tp_clip_tower_forward_train_embed", "tp_clip_tower_backward_crops" if crop_grad else "tp_clip_tower_backward_embed")
+    return names + sizes
 
 
 class _TowerTrainFunction(torch.autograd.Function):
-    """hidden_states 12 / 16 / 22 / 23 with the last K layers under autograd.  Inputs after the first five are the 16 K parameters of
-    the trainable layers, in _lib.CLIP_TOWER_LAYER_FIELDS order, layer 23 - K first; with ``tower.train_embeddings`` (K = 23) the five
-    embedding-stage parameters, in _lib.CLIP_TOWER_FIELDS order, come before them.  checkpoint: keep only each trainable layer's
-    checkpoint (include/tokenpacker_b200_clip_tower_ckpt.h) instead of its full saved set; the backward follows the forward's mode."""
+    """hidden_states 12 / 16 / 22 / 23 under autograd, in every training mode of the tower.  Inputs after the first six are the 16 K
+    parameters of the trainable layers, in _lib.CLIP_TOWER_LAYER_FIELDS order, layer 23 - K first; with ``tower.train_embeddings``
+    (K = 23) the five embedding-stage parameters, in _lib.CLIP_TOWER_FIELDS order, come before them.  checkpoint: keep only each run
+    layer's checkpoint instead of its full saved set; the backward follows the forward's mode.  crop_grad (``tower.input_grad``): all
+    23 layers and the embedding stage run whatever K, every layer below the trainable ones only passes its input gradient on, and the
+    crops get their gradient.  ``images`` are the caller's crops: they are cast to bf16 here, so that fp32 crops receive the fp32
+    gradient the kernels accumulate."""
 
     @staticmethod
-    def forward(ctx, tower, x, packed, w, checkpoint, *params):
-        k, n, device = tower.trainable_layers, x.shape[0], x.device
-        embed_saved = None
+    def forward(ctx, tower, images, packed, w, checkpoint, crop_grad, *params):
+        n, device = images.shape[0], images.device
+        embed = crop_grad or tower.train_embeddings
+        k = _lib.CLIP_TOWER_LAYERS if embed else tower.trainable_layers          # the layers the step runs and keeps
+        x = images.to(torch.bfloat16)
+        if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
+            x = x.contiguous()
+        fwd_name, ctx.bwd_name, saved_bytes, ws_bytes, ctx.bwd_ws_bytes = _train_step(checkpoint, embed, crop_grad, n, k)
         outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=torch.bfloat16, device=device) for _ in _OUT_LAYERS)
-        if checkpoint:
-            forward, name = lib.tp_clip_tower_forward_ckpt, "tp_clip_tower_forward_ckpt"
-            saved_bytes, ws_bytes = lib.tp_clip_tower_ckpt_saved_bytes(n, k), lib.tp_clip_tower_workspace_bytes(n)
-        else:
-            forward, name = lib.tp_clip_tower_forward_train, "tp_clip_tower_forward_train"
-            saved_bytes, ws_bytes = lib.tp_clip_tower_train_saved_bytes(n, k), lib.tp_clip_tower_train_workspace_bytes(n, k)
         saved = torch.empty(saved_bytes, dtype=torch.uint8, device=device)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        embed_saved = None
         ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
+        args = (packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0))
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            if tower.train_embeddings:
+            if embed:
                 embed_bytes = lib.tp_clip_tower_embed_saved_bytes(n)
                 embed_saved = torch.empty(embed_bytes, dtype=torch.uint8, device=device)
-                check(lib.tp_clip_tower_forward_train_embed(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), int(checkpoint), ptrs,
-                                                            saved.data_ptr(), saved_bytes, embed_saved.data_ptr(), embed_bytes, ws.data_ptr(),
-                                                            ws_bytes, stream), "tp_clip_tower_forward_train_embed")
+                status = getattr(lib, fwd_name)(*args, int(checkpoint), ptrs, saved.data_ptr(), saved_bytes, embed_saved.data_ptr(), embed_bytes,
+                                                ws.data_ptr(), ws_bytes, stream)
             else:
-                check(forward(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), k, ptrs, saved.data_ptr(), saved_bytes,
-                              ws.data_ptr(), ws_bytes, stream), name)
-        ctx.w, ctx.saved, ctx.k, ctx.n, ctx.params, ctx.checkpoint = w, saved, k, n, params, checkpoint
-        ctx.embed_saved = embed_saved
+                status = getattr(lib, fwd_name)(*args, k, ptrs, saved.data_ptr(), saved_bytes, ws.data_ptr(), ws_bytes, stream)
+            check(status, fwd_name)
+        ctx.w, ctx.saved, ctx.embed_saved, ctx.k, ctx.n, ctx.checkpoint, ctx.crop_grad = w, saved, embed_saved, k, n, checkpoint, crop_grad
+        ctx.trainable_layers, ctx.train_embeddings, ctx.params = tower.trainable_layers, tower.train_embeddings, params
+        ctx.crops_dtype = images.dtype
         ctx.set_materialize_grads(False)                # an output nobody used arrives as None, not as a tensor of zeros
-        # hidden_states[j] is the output of layer j - 1: below the first trainable layer (23 - k) nothing of it depends on a trainable parameter
+        # hidden_states[j] is the output of layer j - 1: below the first layer run (23 - k) nothing of it depends on a trainable parameter
         frozen = [o for o, j in zip(outs, _OUT_LAYERS) if j - 1 < _lib.CLIP_TOWER_LAYERS - k]
         ctx.mark_non_differentiable(*frozen)
         return outs
@@ -96,98 +118,31 @@ class _TowerTrainFunction(torch.autograd.Function):
         k, n, device = ctx.k, ctx.n, ctx.saved.device
         d_outs = [None if g is None else g.to(torch.bfloat16).contiguous() for g in d_outs]
         d_ptrs = (C.c_void_p * 4)(*[None if g is None else g.data_ptr() for g in d_outs])
-        per = len(_lib.CLIP_TOWER_LAYER_FIELDS)
-        grads = [torch.empty_like(p) if ctx.needs_input_grad[_NUM_FN_INPUTS + i] else None for i, p in enumerate(ctx.params)]
-        n_top = len(_lib.CLIP_TOWER_FIELDS) if ctx.embed_saved is not None else 0
-        g_structs = (_lib.TpClipTowerLayerGrads * k)()
-        for t in range(k):
-            g_structs[t] = _lib.TpClipTowerLayerGrads(*[None if g is None else g.data_ptr() for g in grads[n_top + t * per:n_top + (t + 1) * per]])
-        if ctx.embed_saved is not None:
-            e_struct = _lib.TpClipTowerEmbedGrads(*[None if g is None else g.data_ptr() for g in grads[:n_top]])
-            ws_bytes = (lib.tp_clip_tower_ckpt_backward_workspace_bytes if ctx.checkpoint else lib.tp_clip_tower_backward_workspace_bytes)(n, k)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            with torch.cuda.device(device):
-                stream = torch.cuda.current_stream(device).cuda_stream
-                check(lib.tp_clip_tower_backward_embed(C.byref(ctx.w), ctx.saved.data_ptr(), ctx.embed_saved.data_ptr(), n, int(ctx.checkpoint),
-                                                       d_ptrs, g_structs, C.byref(e_struct), ws.data_ptr(), ws_bytes, stream),
-                      "tp_clip_tower_backward_embed")
-            return (None,) * _NUM_FN_INPUTS + tuple(grads)
-        if ctx.checkpoint:
-            backward, name, ws_bytes = lib.tp_clip_tower_backward_ckpt, "tp_clip_tower_backward_ckpt", lib.tp_clip_tower_ckpt_backward_workspace_bytes(n, k)
-        else:
-            backward, name, ws_bytes = lib.tp_clip_tower_backward, "tp_clip_tower_backward", lib.tp_clip_tower_backward_workspace_bytes(n, k)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            check(backward(C.byref(ctx.w), ctx.saved.data_ptr(), n, k, d_ptrs, g_structs, ws.data_ptr(), ws_bytes, stream), name)
-        return (None,) * _NUM_FN_INPUTS + tuple(grads)
-
-
-class _TowerCropGradFunction(torch.autograd.Function):
-    """hidden_states 12 / 16 / 22 / 23 with the crops under autograd (``tower.input_grad``): the whole-tower training pair
-    (tp_clip_tower_forward_train_embed at 23 layers) and tp_clip_tower_backward_crops.  Inputs after the first five are the tower's
-    trainable parameters in _TowerTrainFunction's order; those that require grad get their gradients, every other layer only passes
-    its input gradient on.  ``images`` are the caller's crops: they are cast to bf16 here, so that fp32 crops receive the fp32 gradient
-    the kernels accumulate."""
-
-    @staticmethod
-    def forward(ctx, tower, images, packed, w, checkpoint, *params):
-        k, n, device = _lib.CLIP_TOWER_LAYERS, images.shape[0], images.device
-        x = images.to(torch.bfloat16)
-        if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
-            x = x.contiguous()
-        outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=torch.bfloat16, device=device) for _ in _OUT_LAYERS)
-        if checkpoint:
-            saved_bytes, ws_bytes = lib.tp_clip_tower_ckpt_saved_bytes(n, k), lib.tp_clip_tower_workspace_bytes(n)
-        else:
-            saved_bytes, ws_bytes = lib.tp_clip_tower_train_saved_bytes(n, k), lib.tp_clip_tower_train_workspace_bytes(n, k)
-        embed_bytes = lib.tp_clip_tower_embed_saved_bytes(n)
-        saved = torch.empty(saved_bytes, dtype=torch.uint8, device=device)
-        embed_saved = torch.empty(embed_bytes, dtype=torch.uint8, device=device)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-        ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
-        with torch.cuda.device(device):
-            stream = torch.cuda.current_stream(device).cuda_stream
-            check(lib.tp_clip_tower_forward_train_embed(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), int(checkpoint), ptrs,
-                                                        saved.data_ptr(), saved_bytes, embed_saved.data_ptr(), embed_bytes, ws.data_ptr(),
-                                                        ws_bytes, stream), "tp_clip_tower_forward_train_embed")
-        ctx.w, ctx.saved, ctx.embed_saved, ctx.n, ctx.checkpoint = w, saved, embed_saved, n, checkpoint
-        ctx.trainable_layers, ctx.train_embeddings, ctx.params = tower.trainable_layers, tower.train_embeddings, params
-        ctx.crops_dtype = images.dtype
-        ctx.set_materialize_grads(False)
-        return outs
-
-    @staticmethod
-    def backward(ctx, *d_outs):
-        n, device = ctx.n, ctx.saved.device
-        d_outs = [None if g is None else g.to(torch.bfloat16).contiguous() for g in d_outs]
-        d_ptrs = (C.c_void_p * 4)(*[None if g is None else g.data_ptr() for g in d_outs])
         grads = [torch.empty_like(p) if ctx.needs_input_grad[_NUM_FN_INPUTS + i] else None for i, p in enumerate(ctx.params)]
         ptr = [None if g is None else g.data_ptr() for g in grads]
         n_top = len(_lib.CLIP_TOWER_FIELDS) if ctx.train_embeddings else 0
-        per, first = len(_lib.CLIP_TOWER_LAYER_FIELDS), _lib.CLIP_TOWER_LAYERS - ctx.trainable_layers
-        g_structs = (_lib.TpClipTowerLayerGrads * _lib.CLIP_TOWER_LAYERS)()
+        per, first = len(_lib.CLIP_TOWER_LAYER_FIELDS), k - ctx.trainable_layers
+        g_structs = (_lib.TpClipTowerLayerGrads * k)()
         for t in range(ctx.trainable_layers):
             g_structs[first + t] = _lib.TpClipTowerLayerGrads(*ptr[n_top + t * per:n_top + (t + 1) * per])
-        e_struct = _lib.TpClipTowerEmbedGrads(*ptr[:n_top]) if n_top else _lib.TpClipTowerEmbedGrads()
         f32 = ctx.crops_dtype == torch.float32
         d_crops = None
-        if ctx.needs_input_grad[1]:
+        if ctx.crop_grad:
             d_crops = torch.empty((n, 3, _IMAGE, _IMAGE), dtype=torch.float32 if f32 else torch.bfloat16, device=device)
-        k = _lib.CLIP_TOWER_LAYERS
-        ws_bytes = (lib.tp_clip_tower_ckpt_backward_workspace_bytes if ctx.checkpoint else lib.tp_clip_tower_backward_workspace_bytes)(n, k)
+        bwd_name, ws_bytes = ctx.bwd_name, ctx.bwd_ws_bytes
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
         with torch.cuda.device(device):
             stream = torch.cuda.current_stream(device).cuda_stream
-            if d_crops is not None:
-                check(lib.tp_clip_tower_backward_crops(C.byref(ctx.w), ctx.saved.data_ptr(), ctx.embed_saved.data_ptr(), n, int(ctx.checkpoint),
-                                                       d_ptrs, g_structs, C.byref(e_struct), d_crops.data_ptr(),
-                                                       _lib.TP_CROP_GRAD_F32 if f32 else _lib.TP_CROP_GRAD_BF16, d_crops.stride(0),
-                                                       ws.data_ptr(), ws_bytes, stream), "tp_clip_tower_backward_crops")
+            if ctx.embed_saved is None:
+                status = getattr(lib, bwd_name)(C.byref(ctx.w), ctx.saved.data_ptr(), n, k, d_ptrs, g_structs, ws.data_ptr(), ws_bytes, stream)
             else:
-                check(lib.tp_clip_tower_backward_embed(C.byref(ctx.w), ctx.saved.data_ptr(), ctx.embed_saved.data_ptr(), n, int(ctx.checkpoint),
-                                                       d_ptrs, g_structs, C.byref(e_struct), ws.data_ptr(), ws_bytes, stream),
-                      "tp_clip_tower_backward_embed")
+                e_struct = _lib.TpClipTowerEmbedGrads(*ptr[:n_top])
+                args = (C.byref(ctx.w), ctx.saved.data_ptr(), ctx.embed_saved.data_ptr(), n, int(ctx.checkpoint), d_ptrs, g_structs,
+                        C.byref(e_struct))
+                if d_crops is not None:
+                    args += (d_crops.data_ptr(), _lib.TP_CROP_GRAD_F32 if f32 else _lib.TP_CROP_GRAD_BF16, d_crops.stride(0))
+                status = getattr(lib, bwd_name)(*args, ws.data_ptr(), ws_bytes, stream)
+            check(status, bwd_name)
         if d_crops is not None and not f32 and ctx.crops_dtype != torch.bfloat16:
             d_crops = d_crops.to(ctx.crops_dtype)
         return (None, d_crops) + (None,) * (_NUM_FN_INPUTS - 2) + tuple(grads)
@@ -400,22 +355,21 @@ class CLIPVisionTowerB200(nn.Module):
         train_params = self._trainable_params() if torch.is_grad_enabled() else []
         train = any(p.requires_grad for p in train_params)
         crop_grad = self._input_grad and torch.is_grad_enabled() and images.requires_grad
-        if crop_grad:
-            if not images.is_cuda:
-                raise RuntimeError("tokenpacker_b200 has no CPU path: crops must be CUDA tensors on an H100")
-            if images.shape[0] == 0:
-                raise ValueError("input_grad needs at least one crop")
-            with torch.cuda.device(images.device):
-                packed, (w, _) = self._packed_weights(images.device)
-                return _TowerCropGradFunction.apply(self, images, packed, self._live_weights(w, train_params, images.device),
-                                                    wants_gradient_checkpointing(self.vision_model), *train_params)
-        if torch.is_grad_enabled() and (images.requires_grad or (self.trainable_layers == 0 and any(p.requires_grad for p in self._params()))):
+        if not crop_grad and torch.is_grad_enabled() and (
+                images.requires_grad or (self.trainable_layers == 0 and any(p.requires_grad for p in self._params()))):
             raise NotImplementedError("CLIPVisionTowerB200 is forward only (the tower is frozen in every TokenPacker recipe): run it under "
                                       "torch.no_grad(), or detach the crops and freeze the tower's parameters")
         if not images.is_cuda:
             raise RuntimeError("tokenpacker_b200 has no CPU path: crops must be CUDA tensors on an H100")
         n = images.shape[0]
+        if crop_grad and n == 0:
+            raise ValueError("input_grad needs at least one crop")
         device = images.device
+        if n > 0 and (crop_grad or train):
+            with torch.cuda.device(device):
+                packed, (w, _) = self._packed_weights(device)
+                return _TowerTrainFunction.apply(self, images, packed, self._live_weights(w, train_params, device),
+                                                 wants_gradient_checkpointing(self.vision_model), crop_grad, *train_params)
         f16 = self.dtype == torch.float16
         outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=self.dtype, device=device) for _ in _OUT_LAYERS)
         if n == 0:
@@ -425,9 +379,6 @@ class CLIPVisionTowerB200(nn.Module):
             if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
                 x = x.contiguous()
             packed, (w, _) = self._packed_weights(device)
-            if train:
-                return _TowerTrainFunction.apply(self, x, packed, self._live_weights(w, train_params, device),
-                                                 wants_gradient_checkpointing(self.vision_model), *train_params)
             ws_bytes = lib.tp_clip_tower_workspace_bytes(n)
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
             ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
