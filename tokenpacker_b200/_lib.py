@@ -4,7 +4,8 @@ There is deliberately no fallback: if the shared library is missing the import f
 Signatures mirror include/tokenpacker_b200.h, include/tokenpacker_b200_hd_u8.h, include/tokenpacker_b200_clip_u8.h,
 include/tokenpacker_b200_input_grad.h, include/tokenpacker_b200_layers.h, include/tokenpacker_b200_clip_tower.h,
 include/tokenpacker_b200_clip_tower_f16.h, include/tokenpacker_b200_clip_tower_train.h, include/tokenpacker_b200_clip_tower_ckpt.h,
-include/tokenpacker_b200_clip_tower_embed.h, include/tokenpacker_b200_clip_tower_crop_grad.h, include/tokenpacker_b200_jpeg.h and include/tokenpacker_b200_png.h one to one.
+include/tokenpacker_b200_clip_tower_embed.h, include/tokenpacker_b200_clip_tower_crop_grad.h, include/tokenpacker_b200_clip_tower_interleaved.h,
+include/tokenpacker_b200_jpeg.h and include/tokenpacker_b200_png.h one to one.
 """
 from __future__ import annotations
 
@@ -191,6 +192,15 @@ CLIP_TOWER_F16_SIGNATURES = {
                                             C.POINTER(C.c_void_p), C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
+# the same for include/tokenpacker_b200_clip_tower_interleaved.h (the four hidden states side by side in one [N, 577, 4096] buffer)
+CLIP_TOWER_INTERLEAVED_SIGNATURES = {
+    "tp_clip_tower_forward_interleaved": (C.c_int, [C.c_void_p, C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
+                                                    C.c_void_p, C.c_size_t, C.c_void_p]),
+    "tp_clip_tower_forward_interleaved_f16": (C.c_int, [C.c_void_p, C.POINTER(TpClipTowerWeights), C.c_void_p, C.c_int, C.c_int64, C.c_int64,
+                                                        C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+}
+
+
 # the same for include/tokenpacker_b200_clip_tower_train.h (training the last K layers of the tower)
 class TpClipTowerLayerGrads(C.Structure):
     """tp_clip_tower_layer_grads: one gradient destination per parameter of a layer (None: not wanted)."""
@@ -337,7 +347,7 @@ def _load():
             "(or `python -c 'import __graft_entry__ as g; g.build()'`). There is no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (restype, argtypes) in {**SIGNATURES, **HD_U8_SIGNATURES, **CLIP_U8_SIGNATURES, **INPUT_GRAD_SIGNATURES,
-                                      **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES,
+                                      **LAYERS_SIGNATURES, **CLIP_TOWER_SIGNATURES, **CLIP_TOWER_F16_SIGNATURES, **CLIP_TOWER_INTERLEAVED_SIGNATURES,
                                       **CLIP_TOWER_TRAIN_SIGNATURES, **CLIP_TOWER_CKPT_SIGNATURES,
                                       **CLIP_TOWER_EMBED_SIGNATURES, **CROP_GRAD_SIGNATURES, **JPEG_SIGNATURES, **PNG_SIGNATURES}.items():
         fn = getattr(lib, name)          # AttributeError here = ABI mismatch: fail loudly

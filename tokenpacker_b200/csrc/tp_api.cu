@@ -18,6 +18,7 @@
 #include "../../include/tokenpacker_b200_clip_tower_ckpt.h"
 #include "../../include/tokenpacker_b200_clip_tower_embed.h"
 #include "../../include/tokenpacker_b200_clip_tower_crop_grad.h"
+#include "../../include/tokenpacker_b200_clip_tower_interleaved.h"
 #include "../../include/tokenpacker_b200_clip_u8.h"
 #include "../../include/tokenpacker_b200_hd_u8.h"
 #include "../../include/tokenpacker_b200_input_grad.h"

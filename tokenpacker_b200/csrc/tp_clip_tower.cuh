@@ -133,15 +133,16 @@ __global__ void clip_embed_preln_kernel(T* __restrict__ x, long long rows, const
 
 // y = Tp(LayerNorm(x) * gamma + beta), one warp per row of [rows, 1024]: layer_norm1 (x: the bf16 / f16 hidden state) / layer_norm2 (x:
 // the fp32 mid-layer residual) of a layer, as an explicit pass (statistics from the row itself, in fp32) so that the following linear
-// reads its weights as they are.  Tp: the tower's storage type (gamma, beta and y).
+// reads its weights as they are.  Tp: the tower's storage type (gamma, beta and y).  ldx: elements between x's rows (1024, or 4096 when
+// x is a hidden state stored into the interleaved output of tp_clip_tower_forward_interleaved); y is dense.
 template <typename T, typename Tp = __nv_bfloat16>
-__global__ void clip_layernorm_kernel(const T* __restrict__ x, long long rows, const Tp* __restrict__ gamma, const Tp* __restrict__ beta,
-                                      Tp* __restrict__ y) {
+__global__ void clip_layernorm_kernel(const T* __restrict__ x, long long ldx, long long rows, const Tp* __restrict__ gamma,
+                                      const Tp* __restrict__ beta, Tp* __restrict__ y) {
   const long long row = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
   float e[32];
-  clip_load_row(x + row * 1024, e, lane);
+  clip_load_row(x + row * ldx, e, lane);
   clip_ln_row_store(e, gamma, beta, y + row * 1024, lane);
 }
 

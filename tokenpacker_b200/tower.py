@@ -156,6 +156,12 @@ def wants_gradient_checkpointing(vision_model: nn.Module) -> bool:
     return any(bool(getattr(m, "gradient_checkpointing", False)) and m.training for m in vision_model.modules())
 
 
+def _check_crops(images):
+    if not isinstance(images, torch.Tensor) or images.dim() != 4 or tuple(images.shape[1:]) != (3, _IMAGE, _IMAGE):
+        shape = tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__
+        raise ValueError(f"expected crops [N,3,336,336], got {shape}")
+
+
 def _check_config(cfg):
     want = {"hidden_size": 1024, "intermediate_size": 4096, "num_attention_heads": 16, "patch_size": 14, "image_size": 336,
             "hidden_act": "quick_gelu", "num_channels": 3}
@@ -349,9 +355,7 @@ class CLIPVisionTowerB200(nn.Module):
         gradient checkpointing 23 x 1.2 MB per crop plus 23 x 6.3 MB (and the 1.86 MB per crop).  Checkpointing follows
         ``wants_gradient_checkpointing``, which needs the wrapped model in training mode: an attribution run on an eval-mode model keeps
         the full saved sets."""
-        if not isinstance(images, torch.Tensor) or images.dim() != 4 or tuple(images.shape[1:]) != (3, _IMAGE, _IMAGE):
-            shape = tuple(images.shape) if isinstance(images, torch.Tensor) else type(images).__name__
-            raise ValueError(f"expected crops [N,3,336,336], got {shape}")
+        _check_crops(images)
         train_params = self._trainable_params() if torch.is_grad_enabled() else []
         train = any(p.requires_grad for p in train_params)
         crop_grad = self._input_grad and torch.is_grad_enabled() and images.requires_grad
@@ -370,24 +374,45 @@ class CLIPVisionTowerB200(nn.Module):
                 packed, (w, _) = self._packed_weights(device)
                 return _TowerTrainFunction.apply(self, images, packed, self._live_weights(w, train_params, device),
                                                  wants_gradient_checkpointing(self.vision_model), crop_grad, *train_params)
-        f16 = self.dtype == torch.float16
         outs = tuple(torch.empty((n, _TOKENS, 1024), dtype=self.dtype, device=device) for _ in _OUT_LAYERS)
-        if n == 0:
-            return outs
-        with torch.cuda.device(device):
-            x = images if f16 and images.dtype in (torch.bfloat16, torch.float16) else images.to(self.dtype)
-            if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
-                x = x.contiguous()
-            packed, (w, _) = self._packed_weights(device)
-            ws_bytes = lib.tp_clip_tower_workspace_bytes(n)
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-            ptrs = (C.c_void_p * 4)(*[o.data_ptr() for o in outs])
-            stream = torch.cuda.current_stream(device).cuda_stream
-            if f16:
-                crops_dtype = _lib.TP_CLIP_CROPS_F16 if x.dtype == torch.float16 else _lib.TP_CLIP_CROPS_BF16
-                check(lib.tp_clip_tower_forward_f16(packed.data_ptr(), C.byref(w), x.data_ptr(), crops_dtype, n, x.stride(0), ptrs, ws.data_ptr(),
-                                                    ws_bytes, stream), "tp_clip_tower_forward_f16")
-            else:
-                check(lib.tp_clip_tower_forward(packed.data_ptr(), C.byref(w), x.data_ptr(), n, x.stride(0), ptrs, ws.data_ptr(), ws_bytes,
-                                                stream), "tp_clip_tower_forward")
+        if n > 0:
+            with torch.cuda.device(device):
+                packed, (w, _) = self._packed_weights(device)
+                self._forward(images, packed, w, (C.c_void_p * 4)(*[o.data_ptr() for o in outs]), interleaved=False)
         return outs
+
+    def interleaved_hidden_states(self, images: torch.Tensor) -> torch.Tensor:
+        """images as for ``hidden_states``.  Returns hidden_states 12, 16, 22 and 23 side by side in one [N, 577, 4096] tensor of the
+        tower's dtype (include/tokenpacker_b200_clip_tower_interleaved.h): columns 1024 j .. 1024 j + 1023 hold hidden_states[(12, 16,
+        22, 23)[j]] with the bits ``hidden_states`` gives.  That is ``torch.cat(tower.hidden_states(images), dim=2)``, LLaVA's
+        ``feature_select`` concatenation, written by the tower in place: one buffer instead of two, and no copy.
+        Inference only: under grad mode, crops or tower parameters that require grad are refused (``hidden_states`` trains)."""
+        _check_crops(images)
+        if torch.is_grad_enabled() and (images.requires_grad or any(p.requires_grad for p in self._params())):
+            raise NotImplementedError("interleaved_hidden_states is inference only: run it under torch.no_grad() (as LLaVA's "
+                                      "CLIPVisionTower.forward does), or train through hidden_states")
+        if not images.is_cuda:
+            raise RuntimeError("tokenpacker_b200 has no CPU path: crops must be CUDA tensors on an H100")
+        n, device = images.shape[0], images.device
+        out = torch.empty((n, _TOKENS, len(_OUT_LAYERS) * 1024), dtype=self.dtype, device=device)
+        if n > 0:
+            with torch.cuda.device(device):
+                packed, (w, _) = self._packed_weights(device)
+                self._forward(images, packed, w, out.data_ptr(), interleaved=True)
+        return out
+
+    def _forward(self, images, packed, w, dest, interleaved: bool):
+        """The inference forward over n > 0 crops into dest: the four outputs' pointers, or the interleaved output's."""
+        f16 = self.dtype == torch.float16
+        n, device = images.shape[0], images.device
+        x = images if f16 and images.dtype in (torch.bfloat16, torch.float16) else images.to(self.dtype)
+        if not (x.stride(3) == 1 and x.stride(2) == _IMAGE and x.stride(1) == _IMAGE * _IMAGE and x.stride(0) >= 3 * _IMAGE * _IMAGE):
+            x = x.contiguous()
+        ws_bytes = lib.tp_clip_tower_workspace_bytes(n)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        stream = torch.cuda.current_stream(device).cuda_stream
+        name = "tp_clip_tower_forward" + ("_interleaved" if interleaved else "") + ("_f16" if f16 else "")
+        crops = (x.data_ptr(),)
+        if f16:
+            crops += (_lib.TP_CLIP_CROPS_F16 if x.dtype == torch.float16 else _lib.TP_CLIP_CROPS_BF16,)
+        check(getattr(lib, name)(packed.data_ptr(), C.byref(w), *crops, n, x.stride(0), dest, ws.data_ptr(), ws_bytes, stream), name)
