@@ -323,7 +323,9 @@ int build_pair_group(const GemmItem* items, int count, int sms, const FrontWork*
     const GemmItem& it = items[i];
     GemmProblem& p = g.p[i];
     if (it.kind == 1) {
-      if (it.N != kC || it.K != kC || it.a2 == nullptr || it.b2 == nullptr || (it.attn.s != 2 && it.attn.s != 4)) return TP_ERR_INVALID_ARGUMENT;
+      if (it.N != kC || it.K != kC || it.a2 == nullptr || it.b2 == nullptr || (it.attn.s != 2 && it.attn.s != 4) ||
+          it.attn.stats_slots != kAttnSlots)
+        return TP_ERR_INVALID_ARGUMENT;
       TP_TRY(make_map_2d(&p.tmap_a, it.a.ptr, it.M, it.K, it.a.ld, kBlockM));
       TP_TRY(make_map_2d(&p.tmap_a2, it.a2, it.M, it.K, it.a.ld, kBlockM));
       TP_TRY(make_map_2d(&p.tmap_b, it.b, it.N, it.K, it.ldb, Cfg::kTileN / 2));   // the head pair's 256 weight rows: 128 per CTA

@@ -23,7 +23,7 @@
 //               kernel's scattered segment rows and fp32 outputs) and KV-attention tiles: each warp turns its fragments into
 //               thread == output row form (lanes 0-15: column half 0, lanes 16-31: column half 1 of the warp's 16 rows) through a
 //               2 KiB shared-memory transpose (32 columns at a time), then fused per-row / per-column math and 16-byte global stores
-//               (epilogue_tile) or the window softmax (attn_scores / attn_pv)
+//               (epilogue_tile).  KV-attention tiles: the window softmax on the fragments (attn_scores / attn_pv)
 //   warps 8, 9  store warps of the pair kernel (one per column half): wait for a finished slab on an mbarrier, issue its TMA
 //               store(s), hand the buffer back, and — for GEMMs that other GEMMs of the same launch depend on — publish each
 //               finished tile to a global counter.  The epilogue warps never wait for a store.
@@ -102,7 +102,7 @@ constexpr int kScratchBytes = kNumEpiWarps * kScratchBytesPerWarp;
 
 // Pair kernel: tile row of epilogue thread (warpgroup wg, quarter, lane): the 16 rows whose wgmma fragments warp `quarter` of
 // warpgroup wg holds, once for each column half (lanes 0-15: half 0, lanes 16-31: half 1: epi_half), so the fragment -> row
-// transpose never leaves the warp.  Windows of 4 or 16 consecutive rows stay inside 16 consecutive lanes.
+// transpose never leaves the warp.
 __device__ __forceinline__ int epi_row(int wg, int quarter, uint32_t lane) {
   return 64 * wg + 16 * quarter + static_cast<int>(lane & 15u);
 }
@@ -243,9 +243,8 @@ __device__ __forceinline__ long long window_major_row(long long row, int s) {
   return n * 576 + ((hb * (24 / s) + wb) * s + hi) * s + wi;
 }
 
-// (mean, rstd) of a LayerNorm row from its per-128-column (mean, M2) pairs, combined Chan-style in fixed order
-__device__ __forceinline__ void ln_row_stats(const float* stats, long long row, int slots, float inv_dim, float eps, float& mu, float& rstd) {
-  const float2* st = reinterpret_cast<const float2*>(stats) + row * slots;
+// (mean, rstd) of a LayerNorm row from its per-128-column (mean, M2) pairs st[0 .. slots), combined Chan-style in fixed order
+__device__ __forceinline__ void ln_stats_combine(const float2* st, int slots, float inv_dim, float eps, float& mu, float& rstd) {
   float t1 = 0.f, m2 = 0.f;
   for (int i = 0; i < slots; ++i) t1 = __fadd_rn(t1, st[i].x);
   const float inv_slots = rcp_rn_normal(static_cast<float>(slots));      // slots in [1, 64], inv_dim in [2^-13, 1]: call-free
@@ -259,6 +258,9 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, long long row, 
   }
   const float var = __fmul_rn(fmaf(between, __fmul_rn(inv_slots, rcp_rn_normal(inv_dim)), m2), inv_dim);
   rstd = rsqrtf(__fadd_rn(var, eps));
+}
+__device__ __forceinline__ void ln_row_stats(const float* stats, long long row, int slots, float inv_dim, float eps, float& mu, float& rstd) {
+  ln_stats_combine(reinterpret_cast<const float2*>(stats) + row * slots, slots, inv_dim, eps, mu, rstd);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -423,12 +425,21 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, int M, int
 // (builder.py:122-130 == nn.MultiheadAttention, L = 1 query, S = s*s keys per window, 8 heads x 128).
 //   A tile = 256 window-major rows (CTA pair) x TWO heads, in two accumulator phases of the ordinary 256 x 256 x K pipeline:
 //     phase K: k' = y_k . (gamma_k W_ik)^T for the two heads  -> epilogue: folded LayerNorm, dot with the window's q' (already scaled
-//              by 1/sqrt 128), softmax over the s*s consecutive lanes of the window (warp shuffles)  -> p stays in a register
-//     phase V: v' = y_v . (gamma_v W_iv)^T                     -> epilogue: folded LayerNorm, p * v', halving exchange over the window's
-//              lanes, store the window's 128 context channels of the head
+//              by 1/sqrt 128), softmax over the window's s*s consecutive rows  -> p stays in registers
+//     phase V: v' = y_v . (gamma_v W_iv)^T                     -> epilogue: folded LayerNorm, p * v', summed over the window's rows,
+//              store the window's 128 context channels of each head
 //   Both phases use the same accumulator registers one after the other; the producer keeps the ring full in the meantime.
-//   Thread == key row; column half (lanes 0-15 / 16-31 of every epilogue warp) == head of the pair.  k' and v' never exist in
-//   memory (fp32, unrounded, in registers): the [R,1024] x 2 round trip through HBM and the separate attention kernel are gone.
+//   k' and v' never exist in memory (fp32, unrounded, in registers): the [R,1024] x 2 round trip through HBM and the separate
+//   attention kernel are gone.
+//   Both epilogues work on the wgmma m64n256 fragments where they are: lane (g = lane / 4, q = lane % 4) of a warp holds rows g and
+//   g + 8 of the warp's 16 rows, acc[h][4 j + 2 r + e] = row g + 8 r, column 8 j + 2 q + e of column half h == head h of the pair.
+//   A window is W = s*s consecutive rows, W-aligned: for s = 2 the rows g = 4 a .. 4 a + 3 of one r (lanes xor 4, 8), for s = 4
+//   all 16 rows of the warp (the lane's two rows, lanes xor 4, 8, 16).
+//   Order of the sums: a row's score is the lane's 32 products in column order, then the 4 lanes of the row (xor 1, then xor 2);
+//   the softmax denominator and the context sums are pairwise trees over the window's rows (s = 4: the lane's rows g + g + 8 first).
+//   What the epilogues read after the mainloop is fetched while the tensor pipe is busy: the (mean, M2) slots of the warp's rows of
+//   y_k and y_v into registers (attn_load_stats), the q' rows of the CTA's windows into the (otherwise unused) transpose scratch
+//   (attn_load_q).
 // ------------------------------------------------------------------------------------------------
 struct AttnParams {
   const __nv_bfloat16* qp;      // [Q, 1024] q', row = window index (= query index), scaled
@@ -440,7 +451,7 @@ struct AttnParams {
   const float* wsum_v;
   const float* cst_v;
   int s;                        // scale factor: W = s*s consecutive rows per window (2 or 4)
-  int stats_slots;
+  int stats_slots;              // = kAttnSlots (host-checked)
   float ln_inv_dim, ln_eps;
   int* done_counter;            // ctx row blocks of 256 queries: counter[(m_blk * 256 / W) / 256] += 1 per (CTA, head pair)
   // dependencies of a tile: the raster row blocks of y_k / y_v covering the crops it touches, and its queries' q' row block
@@ -451,88 +462,209 @@ struct AttnParams {
   int q_target;
 };
 
-__device__ __forceinline__ float bf16x2_get(const uint4& v, int i) {      // i in [0, 8)
-  const uint32_t w = i < 4 ? (i < 2 ? v.x : v.y) : (i < 6 ? v.z : v.w);
-  return (i & 1) ? bf16_hi(w) : bf16_lo(w);
+constexpr int kAttnSlots = 8;         // (mean, M2) slots of a y_k / y_v row: 1024 columns / 128
+constexpr int kAttnQBytes = 512;      // q' of one window in the scratch: the tile's two heads x 128 bf16
+static_assert(kBlockM / 4 * kAttnQBytes <= kScratchBytes, "q' of a CTA's windows (s = 2) fits the transpose scratch");
+
+// The (mean, M2) slots of the warp's 16 rows of y_k or y_v: lane l loads slots 4 (l / 16) .. + 3 of row row_w0 + l % 16 (zeros past
+// M).  Phase K's are issued before its MMAs, phase V's before its epilogue, so that both land while the tensor pipe is busy.
+__device__ __forceinline__ void attn_load_stats(const float* stats, int M, int row_w0, float4 (&st)[2]) {
+  const uint32_t lane = lane_id();
+  const int row = row_w0 + static_cast<int>(lane & 15u);
+  const float4* src = reinterpret_cast<const float4*>(stats + static_cast<long long>(row) * (2 * kAttnSlots)) + 2 * (lane >> 4);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) st[i] = row < M ? __ldcg(src + i) : make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
-// Phase K epilogue: returns this row's softmax weight p for head `head`.  s_vec: wsum | cst of the tile's two heads (col_slot).
-__device__ __forceinline__ float attn_scores(const AttnParams& at, int M, const float (&acc)[2][64], uint32_t scratch, int row, int head,
-                                             int half, const float* s_vec) {
+// (mu, rstd) of row row_w0 + l % 16 in lanes l < 16 from attn_load_stats (0, 0 past M: k' = v' = the folded constant there)
+__device__ __forceinline__ void attn_row_stats(const AttnParams& at, const float4 (&st)[2], int M, int row_w0, float& mu, float& rstd) {
+  float4 hi[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    hi[i].x = __shfl_down_sync(0xffffffffu, st[i].x, 16);
+    hi[i].y = __shfl_down_sync(0xffffffffu, st[i].y, 16);
+    hi[i].z = __shfl_down_sync(0xffffffffu, st[i].z, 16);
+    hi[i].w = __shfl_down_sync(0xffffffffu, st[i].w, 16);
+  }
+  const float2 v[kAttnSlots] = {make_float2(st[0].x, st[0].y), make_float2(st[0].z, st[0].w), make_float2(st[1].x, st[1].y),
+                                make_float2(st[1].z, st[1].w), make_float2(hi[0].x, hi[0].y), make_float2(hi[0].z, hi[0].w),
+                                make_float2(hi[1].x, hi[1].y), make_float2(hi[1].z, hi[1].w)};
+  mu = 0.f;
+  rstd = 0.f;
+  if (row_w0 + static_cast<int>(lane_id() & 15u) < M) ln_stats_combine(v, kAttnSlots, at.ln_inv_dim, at.ln_eps, mu, rstd);
+}
+
+// q' of the CTA's 128 / W windows for the tile's two heads into the transpose scratch (cp.async; issued before phase K's MMAs, landed
+// by col_vectors_ready): window wl at scratch + wl * kAttnQBytes, its 16-byte piece u (channels 8 u ..) XOR-swizzled to
+// (u ^ (wl & 7)) * 16, so that the two windows one warp instruction reads (s = 2) sit in different banks; zeros past the last window
+__device__ __forceinline__ void attn_load_q(const AttnParams& at, int M, int row_cta0, int n_blk, uint32_t scratch, int epi_tid) {
   const int W = at.s * at.s;
-  const bool row_ok = row < M;
-  float mu = 0.f, rstd = 0.f;
-  if (row_ok) ln_row_stats(at.stats_k, row, at.stats_slots, at.ln_inv_dim, at.ln_eps, mu, rstd);
-  const long long window = row / W;
-  const float* wsum = s_vec + col_slot<256>(0, half * 128);
-  const float* cst = s_vec + col_slot<256>(1, half * 128);
-  const uint4* qrow = reinterpret_cast<const uint4*>(at.qp + window * 1024 + head * 128);
-  uint32_t r[32];
-  float score = 0.f;
+  const long long win0 = row_cta0 / W, n_win = M / W;
+  for (int i = epi_tid; i < (kBlockM / W) * 32; i += kEpiThreads) {
+    const int wl = i >> 5, u = i & 31;
+    const long long w = win0 + wl;
+    const bool ok = w < n_win;
+    cp_async_16(scratch + static_cast<uint32_t>(wl * kAttnQBytes + ((u ^ (wl & 7)) << 4)), at.qp + (ok ? w : 0) * 1024 + n_blk * 256 + u * 8,
+                ok ? 16u : 0u);
+  }
+}
+
+// Phase K epilogue: p[h][r] = the softmax weight of the lane's row g + 8 r for head h of the pair.
+//   mu_own / rstd_own: attn_row_stats of y_k (lanes 0-15); rloc_w0: CTA row of the warp's first row; scratch: the q' rows
+//   (attn_load_q); s_vec: wsum | cst of the tile's two heads (col_slot)
+__device__ __forceinline__ void attn_scores(const AttnParams& at, const float (&acc)[2][64], float mu_own, float rstd_own, int rloc_w0,
+                                            uint32_t scratch, const float* s_vec, float (&p)[2][2]) {
+  const uint32_t lane = lane_id();
+  const uint32_t g = lane >> 2, q = lane & 3u;
+  const int W = at.s * at.s;
+  float mu[2], rstd[2];
+  uint32_t qa[2], swz[2];
 #pragma unroll
-  for (int chunk = 0; chunk < 4; ++chunk) {
-    acc_chunk(acc, chunk, scratch, r);
-    uint4 q4[4];
+  for (int r = 0; r < 2; ++r) {
+    mu[r] = __shfl_sync(0xffffffffu, mu_own, static_cast<int>(g) + 8 * r);
+    rstd[r] = __shfl_sync(0xffffffffu, rstd_own, static_cast<int>(g) + 8 * r);
+    const int wl = (rloc_w0 + static_cast<int>(g) + 8 * r) / W;
+    qa[r] = scratch + static_cast<uint32_t>(wl * kAttnQBytes) + 4u * q;
+    swz[r] = static_cast<uint32_t>(wl & 7);
+  }
+  const uint32_t sa = smem_u32(s_vec + col_slot<256>(0, 0)), sb = smem_u32(s_vec + col_slot<256>(1, 0));
+  float part[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 #pragma unroll
-    for (int i = 0; i < 4; ++i) q4[i] = row_ok ? __ldg(qrow + chunk * 4 + i) : make_uint4(0u, 0u, 0u, 0u);
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-    for (int c = 0; c < 32; ++c) {
-      const float kf = fmaf(rstd, fmaf(-mu, wsum[chunk * 32 + c], __uint_as_float(r[c])), cst[chunk * 32 + c]);
-      score = fmaf(bf16x2_get(q4[c >> 3], c & 7), kf, score);
+    for (int j = 0; j < 16; ++j) {
+      const uint32_t c = static_cast<uint32_t>(h * 128 + 8 * j + (h ? kColPad : 0)) + 2u * q;    // col_slot offset
+      float w0, w1, c0, c1;
+      upk2(lds_f2(sa + c * 4u), w0, w1);
+      upk2(lds_f2(sb + c * 4u), c0, c1);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const uint32_t qw = lds_u32(qa[r] + (((16u * h + j) ^ swz[r]) << 4));
+        const float k0 = fmaf(rstd[r], fmaf(-mu[r], w0, acc[h][4 * j + 2 * r]), c0);
+        const float k1 = fmaf(rstd[r], fmaf(-mu[r], w1, acc[h][4 * j + 2 * r + 1]), c1);
+        part[h][r] = fmaf(bf16_lo(qw), k0, part[h][r]);
+        part[h][r] = fmaf(bf16_hi(qw), k1, part[h][r]);
+      }
+    }
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      part[h][r] += __shfl_xor_sync(0xffffffffu, part[h][r], 1);
+      part[h][r] += __shfl_xor_sync(0xffffffffu, part[h][r], 2);
+    }
+  // softmax over the window's W rows (every lane of the window gets the same max and denominator: a + b == b + a)
+  if (W == 4) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float mx = part[h][r];
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 4));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 8));
+        const float e = __expf(part[h][r] - mx);
+        float den = e + __shfl_xor_sync(0xffffffffu, e, 4);
+        den += __shfl_xor_sync(0xffffffffu, den, 8);
+        p[h][r] = e * rcp_rn_normal(den);               // den in [1, 4]: the correctly rounded 1 / den, without a call
+      }
+  } else {                                              // W == 16
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = fmaxf(part[h][0], part[h][1]);
+#pragma unroll
+      for (int off = 4; off < 32; off <<= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+      const float e0 = __expf(part[h][0] - mx), e1 = __expf(part[h][1] - mx);
+      float den = e0 + e1;
+#pragma unroll
+      for (int off = 4; off < 32; off <<= 1) den += __shfl_xor_sync(0xffffffffu, den, off);
+      const float inv = rcp_rn_normal(den);             // den in [1, 16]
+      p[h][0] = e0 * inv;
+      p[h][1] = e1 * inv;
     }
   }
-  // softmax over the W keys of my window = W consecutive lanes (W divides 16: windows never straddle a 16-lane half, see epi_row)
-  float mx = score;
-  for (int off = 1; off < W; off <<= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-  const float e = __expf(score - mx);
-  float den = e;
-  for (int off = 1; off < W; off <<= 1) den += __shfl_xor_sync(0xffffffffu, den, off);
-  return e * rcp_rn_normal(den);                    // den in [1, 16]: the correctly rounded 1 / den, without a call
 }
 
-// Phase V epilogue: ctx = sum over the window's lanes of p * v'.  Halving exchange: after log2(W) steps each lane holds 32 / W
-// channels of the chunk.
-__device__ __forceinline__ void attn_pv(const AttnParams& at, int M, const float (&acc)[2][64], uint32_t scratch, int row, int head, int half,
-                                        float p, const float* s_vec) {
-  const int W = at.s * at.s;
-  const bool row_ok = row < M;
+// Phase V epilogue: ctx = sum over the window's rows of p * v'.  Halving exchange: each step sends half of the lane's live values to
+// the partner lane and adds the other half of the partner's, so that afterwards the 4 (s = 2) or 16 (s = 4) lanes of a window hold
+// disjoint shares of its two heads x 128 channels, and store them as bf16 pairs (no value is stored twice).  Four rounds of 4
+// 8-column groups each, so that few values are live at a time; acc itself is only read (the next tile's wgmmas take it over).
+//   mu_own / rstd_own: attn_row_stats of y_v (lanes 0-15); row_w0: global row of the warp's first row
+__device__ __forceinline__ void attn_pv(const AttnParams& at, int M, const float (&acc)[2][64], float mu_own, float rstd_own, int row_w0,
+                                        int n_blk, const float (&p)[2][2], const float* s_vec) {
   const uint32_t lane = lane_id();
-  float mu = 0.f, rstd = 0.f;
-  if (row_ok) ln_row_stats(at.stats_v, row, at.stats_slots, at.ln_inv_dim, at.ln_eps, mu, rstd);
-  const long long window = row / W;
-  const float* wsum = s_vec + col_slot<256>(0, half * 128);
-  const float* cst = s_vec + col_slot<256>(1, half * 128);
-  uint32_t r[32];
+  const uint32_t g = lane >> 2, q = lane & 3u;
+  const int W = at.s * at.s;
+  float mu[2], rstd[2];
 #pragma unroll
-  for (int chunk = 0; chunk < 4; ++chunk) {
-    acc_chunk(acc, chunk, scratch, r);
-    float v[32];
+  for (int r = 0; r < 2; ++r) {
+    mu[r] = __shfl_sync(0xffffffffu, mu_own, static_cast<int>(g) + 8 * r);
+    rstd[r] = __shfl_sync(0xffffffffu, rstd_own, static_cast<int>(g) + 8 * r);
+  }
+  const uint32_t sa = smem_u32(s_vec + col_slot<256>(0, 0)), sb = smem_u32(s_vec + col_slot<256>(1, 0));
+  const bool up4 = (lane & 4u) != 0, up8 = (lane & 8u) != 0, up16 = (lane & 16u) != 0;
+  const int head = 2 * n_blk + (up4 ? 1 : 0);
+  // o[r][e] = p v' of (head h, 8-column group j, row g + 8 r, column 8 j + 2 q + e)
+  auto pv = [&](int h, int j, float (&o)[2][2]) {
+    const uint32_t c = static_cast<uint32_t>(h * 128 + 8 * j + (h ? kColPad : 0)) + 2u * q;    // col_slot offset
+    float w[2], cs[2];
+    upk2(lds_f2(sa + c * 4u), w[0], w[1]);
+    upk2(lds_f2(sb + c * 4u), cs[0], cs[1]);
 #pragma unroll
-    for (int c = 0; c < 32; ++c)
-      v[c] = p * fmaf(rstd, fmaf(-mu, wsum[chunk * 32 + c], __uint_as_float(r[c])), cst[chunk * 32 + c]);
-    int first = 0;                                    // my live values cover channels [first, first + 32 >> steps) of the chunk
+    for (int r = 0; r < 2; ++r)
 #pragma unroll
-    for (int step = 0; step < 4; ++step) {
-      const int off = 1 << step;
-      const int hn = 16 >> step;                      // steps run as a prefix (off < W), so the live count before step k is 32 >> k
-      if (off < W) {
-        const bool up = (lane & off) != 0;            // upper lane of the pair keeps the upper half
+      for (int e = 0; e < 2; ++e) o[r][e] = p[h][r] * fmaf(rstd[r], fmaf(-mu[r], w[e], acc[h][4 * j + 2 * r + e]), cs[e]);
+  };
+  // keep `up ? hi : lo`, add the partner's (lane ^ off) copy of it
+  auto halve = [](float lo, float hi, bool up, int off) {
+    const float send = up ? lo : hi, keep = up ? hi : lo;
+    return keep + __shfl_xor_sync(0xffffffffu, send, off);
+  };
+  if (W == 4) {
+    // window = rows g = 4 a .. 4 a + 3 of one r: xor 4 keeps head up4, xor 8 keeps row g + 8 up8; round jc: groups j = 4 jc .. + 3
+    const int row = row_w0 + static_cast<int>(g) + (up8 ? 8 : 0);
+    __nv_bfloat16* dst = at.ctx + static_cast<long long>(row / 4) * 1024 + head * 128 + 2 * static_cast<int>(q);
 #pragma unroll
-        for (int i = 0; i < hn; ++i) {
-          const float send = up ? v[i] : v[i + hn];
-          const float keep = up ? v[i + hn] : v[i];
-          v[i] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-        }
-        if (up) first += hn;
+    for (int jc = 0; jc < 4; ++jc) {
+      float v[4][2][2];                                 // [j][r][e]
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        float o0[2][2], o1[2][2];
+        pv(0, 4 * jc + jj, o0);
+        pv(1, 4 * jc + jj, o1);
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) v[jj][r][e] = halve(o0[r][e], o1[r][e], up4, 4);
+      }
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const float c0 = halve(v[jj][0][0], v[jj][1][0], up8, 8), c1 = halve(v[jj][0][1], v[jj][1][1], up8, 8);
+        if (row < M) *reinterpret_cast<uint32_t*>(dst + 8 * (4 * jc + jj)) = pack_bf16x2(c0, c1);
       }
     }
-    if (row_ok) {
-      __nv_bfloat16* dst = at.ctx + window * 1024 + head * 128 + chunk * 32 + first;
-      if (W == 4) {
-        *reinterpret_cast<uint4*>(dst) = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-      } else {                                        // W == 16: two channels per lane
-        *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(v[0], v[1]);
+  } else {
+    // W == 16: window = all 16 rows: the lane's two rows first, then xor 4 keeps head up4, xor 8 keeps groups j = 8 up8 + .., xor 16
+    // j = 8 up8 + 4 up16 + ..; round jc: groups jc, jc + 4, jc + 8, jc + 12, of which the lane stores jc + 4 up16 + 8 up8
+    __nv_bfloat16* dst = at.ctx + static_cast<long long>(row_w0 / 16) * 1024 + head * 128 + 2 * static_cast<int>(q);
+#pragma unroll
+    for (int jc = 0; jc < 4; ++jc) {
+      float v[4][2];                                    // [group jc + 4 k][e]
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        float o0[2][2], o1[2][2];
+        pv(0, jc + 4 * k, o0);
+        pv(1, jc + 4 * k, o1);
+#pragma unroll
+        for (int e = 0; e < 2; ++e) v[k][e] = halve(o0[0][e] + o0[1][e], o1[0][e] + o1[1][e], up4, 4);
       }
+      float c[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float a = halve(v[0][e], v[2][e], up8, 8), b = halve(v[1][e], v[3][e], up8, 8);   // groups jc + 8 up8, jc + 4 + 8 up8
+        c[e] = halve(a, b, up16, 16);
+      }
+      const int j = jc + (up16 ? 4 : 0) + (up8 ? 8 : 0);
+      if (row_w0 < M) *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(c[0], c[1]);
     }
   }
 }
@@ -972,6 +1104,7 @@ struct GemmGroup {
   FrontWork front;
 };
 
+
 // __grid_constant__ parameters of tp_gemm2_kernel: the kernel parameter space of sm_90 holds 32764 bytes
 static_assert(sizeof(GemmGroup) + sizeof(PeerStores) <= 32764, "tp_gemm2_kernel's parameter block exceeds the 32 KB limit");
 
@@ -1109,17 +1242,29 @@ tp_gemm2_kernel(const __grid_constant__ GemmGroup grp, const __grid_constant__ P
       const int row = row_tile0 + rloc;
       if (!kTower && pr.kind == 1) {
         const AttnParams& at = pr.attn;
-        const int head = t.n_blk * 2 + half;                 // column half == head of the tile's pair
-        named_bar_sync(kEpiBarrierId, kEpiThreads);          // everyone is done reading the previous tile's vectors
+        const int rloc_w0 = 64 * wg + 16 * (warp_idx & 3);
+        const uint32_t q_scratch = smem_u32(s_scratch);
+        named_bar_sync(kEpiBarrierId, kEpiThreads);          // everyone is done reading the previous tile's vectors and scratch
         stage_col_vectors_async<kTileN>(at.wsum_k, at.cst_k, pr.N, t.n_blk * kTileN, s_col, epi_tid);
+        // the first stage is full: the producer has acquired y_k, y_v, their statistics and q' (tile counters); mma_tile's own wait
+        // on it returns at once
+        mbar_wait(&full_bar[stage], phase);
+        float4 st[2];
+        attn_load_stats(at.stats_k, pr.M, row_tile0 + rloc_w0, st);
+        attn_load_q(at, pr.M, row_tile0, t.n_blk, q_scratch, epi_tid);
         mma_tile<kTileN, 1, 0, 0>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
-        col_vectors_ready();
-        const float p = attn_scores(at, pr.M, acc, scratch, row, head, half, s_col);
+        float mu, rstd;                                      // lanes 0-15: of row row_tile0 + rloc_w0 + lane
+        attn_row_stats(at, st, pr.M, row_tile0 + rloc_w0, mu, rstd);
+        attn_load_stats(at.stats_v, pr.M, row_tile0 + rloc_w0, st);
+        col_vectors_ready();                                 // also the q' copies
+        float p[2][2];
+        attn_scores(at, acc, mu, rstd, rloc_w0, q_scratch, s_col, p);
+        attn_row_stats(at, st, pr.M, row_tile0 + rloc_w0, mu, rstd);
         named_bar_sync(kEpiBarrierId, kEpiThreads);          // everyone is done reading phase K's vectors
         stage_col_vectors_async<kTileN>(at.wsum_v, at.cst_v, pr.N, t.n_blk * kTileN, s_col, epi_tid);
         mma_tile<kTileN, 1, 0, 0>(acc, smem, Cfg::kStageBytes, wg * 8192, Cfg::kABytes, full_bar, empty_bar, kStages, stage, phase, pr.num_k_blocks);
         col_vectors_ready();
-        attn_pv(at, pr.M, acc, scratch, row, head, half, p, s_col);
+        attn_pv(at, pr.M, acc, mu, rstd, row_tile0 + rloc_w0, t.n_blk, p, s_col);
         if (at.done_counter != nullptr) {
           named_bar_sync(kEpiBarrierId, kEpiThreads);       // every epilogue thread's ctx stores are issued ...
           if (epi_tid == 0) {
